@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the `speedseq align` hot path on B200: reads/s ALIGNED + DUP-MARKED (BASELINE.json's metric).
+"""bench.py — throughput of the `speedseq align` hot path on H100: reads/s ALIGNED + DUP-MARKED (BASELINE.json's metric).
 
-One STEP = one run of `bwa mem | samblaster` (/root/reference/bin/speedseq:438-439) over the whole workload: every batch goes
+One STEP = one run of `bwa mem | samblaster` (speedseq's bin/speedseq:438-439) over the whole workload: every batch goes
 through seeding, SA look-up, chaining, seed extension, sort/dedup/patch, insert-size statistics, mate rescue, pairing, MAPQ,
 CIGAR/NM/MD, samblaster's signature / discordant / splitter tests, first-seen-wins duplicate marking against all earlier batches
 of the step, and the three SAM record streams are written (main with 0x400 + MC/MQ, splitters, discordants) — the C-ABI call
@@ -10,19 +10,24 @@ ssq_aligner_* of include/ssq.h, which is what the `bwa` shim drives.
 Workload ("config.workload"): synthetic 2x150 bp paired-end reads (wgsim-like: 0.5 % substitution errors, 0.085 % SNPs, ~2 % of
 reads with a 1-3 bp indel, insert 500+-50; 10 % of the pairs are exact duplicates of earlier pairs under new names, 1 % are
 chimeric: the mate comes from elsewhere) against a seeded synthetic reference with planted repeat families (no real genome
-exists on the box), in batches of 2 M reads (bwa's batch rule at -t 30: 10 Mbp x threads).
+exists on the box), 3 M reads per step in batches of 1 M reads (bwa's batch rule at -t 15: 10 Mbp x threads).  Every batch of a
+step stays resident with its own aligner object (about 20 GB of HBM per 1 M-read batch), which is what bounds a step to 3 M reads
+on an 80 GB H100.
 
   value : reads/s with every batch's FASTQ fields already resident in HBM when the timed region starts; the timed region ends when
           the last batch's SAM text is complete in HBM (CUDA events on the launching streams, max over ranks).
   e2e   : the same metric through the same C-ABI with HOST (pinned) buffers: every batch's names / bases / qualities are copied
           host->device and its three SAM streams device->host inside the timed region.
-  Inputs + scratch per step exceed the 126 MB L2 many times over (config.l2).
+  Inputs + scratch per step exceed the 50 MB L2 many times over (config.l2).
   roofline : the kernel with the largest share of the step among those with a defined byte count (seeding: rank-block bytes
-          dereferenced, counted on the device; SA look-up; text: bytes written + FASTQ bytes read; dup-set: 25 B/pair).
+          dereferenced, counted on the device; SA look-up; text: bytes written + FASTQ bytes read; dup-set: 25 B/pair), against
+          the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s).
   cpu_baseline : the oracle (scalar C restatement of bwa mem + samblaster, oracle/) on all host cores over a bounded sample of
-          the same reads ("port": the reference's bwa/samblaster sources are not vendored in /root/reference).
+          the same reads ("port": speedseq does not vendor the bwa/samblaster sources).
   parity : the GPU streams of that same sample (run as its own batch) compared byte for byte with the oracle's.
 
+The synthetic genome and its index are kept under --cache / SSQ_BENCH_CACHE when given (the tools reuse cache_dir()); by default
+they are built in a temporary directory that is removed when the run ends.  Never in the source tree.  `--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (see dump_outputs()).
 `--impl reference` runs ONLY the CPU arm (rank 0), K steps of a bounded sample each.
 Multi-GPU: batches are dealt to ranks (weak scaling: every rank runs the same number of batches on its own reads), the index is
 replicated; see DESIGN.md §6 for the dup-signature exchange.
@@ -31,6 +36,7 @@ import argparse
 import ctypes as C
 import json
 import os
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -46,6 +52,9 @@ GENOME_LEN = 1000000000  # the largest round size the GPU index builder handles 
 READ_LEN = 150
 SB = dict(exclude_dups=1, add_mate_tags=1, max_split_count=2, min_non_overlap=20)  # bin/speedseq:439 with its defaults (:241-243)
 SB_ARGS = ["--excludeDups", "--addMateTags", "--maxSplitCount", "2", "--minNonOverlap", "20"]
+HBM_GBPS = 3350.0  # H100 SXM data sheet (HBM3); a data-sheet figure, not a measured one
+DUMP_READS_PER_BATCH = 20000  # seeded sample of reads whose main-stream records --dump-outputs writes ...
+DUMP_BYTES = 64 << 20  # ... capped so that all files of all ranks stay within 64 MB
 
 
 # ------------------------------------------------------------------------------------ data ----
@@ -139,6 +148,12 @@ class Batch:
         self.h2d = int(self.seq.numel()) * 2 + (n + 1) * 12 + int(self.name.numel())
 
 
+def cache_dir():
+    """where the tools keep synthetic genomes and their indexes between runs: SSQ_BENCH_CACHE, else a per-user directory in the
+    system temp dir (never the source tree)"""
+    return os.environ.get("SSQ_BENCH_CACHE") or os.path.join(tempfile.gettempdir(), "ssq_bench_cache_%d" % os.getuid())
+
+
 def ensure_reference(cache, genome_len, builder):
     """seeded synthetic genome (8 contigs) + index under `cache`; builder(fasta) makes the five index files"""
     os.makedirs(cache, exist_ok=True)
@@ -177,7 +192,7 @@ def usable_cores():
 
 
 class ClockSampler:
-    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, gpu):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -201,8 +216,9 @@ class ClockSampler:
                 for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[5:9]):
                     if v.strip() == "Active":
                         reasons.add(name)
+        plim = [r[9] for r in rows if len(r) > 9 and r[9].replace(".", "", 1).isdigit()]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": int(rows[0][2]) if rows and rows[0][2].isdigit() else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "reasons": sorted(reasons), "samples": len(sm), "power_limit_w": float(plim[0]) if plim else None}
 
 
 # ---------------------------------------------------------------------------------- CPU arm ----
@@ -235,16 +251,55 @@ def cpu_arm(T, o, oidx, fa, batch, n, threads):
     return n / dt, dt, streams, (t_mem, t_sb)
 
 
+def dump_outputs(d, s, aligners, batches, fa, rank, world):
+    """what the last timed step computed, as a caller of ssq_aligner_* receives it (the three SAM record streams of every batch), in
+    numbers that two builds can be compared by:
+      streams.npy      float64 [batches, 3, 3]: bytes, records and CRC-32 of the main / splitter / discordant stream of each batch
+      main_sample.npy  float64 [batches * S, 8]: for a fixed seeded sample of S reads per batch: batch, read index, then FLAG,
+                       contig index (-1 for '*'), POS, MAPQ, TLEN of the read's first main-stream record and the CRC-32 of all its
+                       main-stream records
+    With several ranks each writes its own files (suffix _rank<r>).  S shrinks below DUMP_READS_PER_BATCH when the batches of all
+    ranks would otherwise take more than DUMP_BYTES."""
+    import zlib
+    os.makedirs(d, exist_ok=True)
+    ann = open(fa + ".ann").read().splitlines()[1:]
+    cid = {l.split()[1]: i for i, l in enumerate(ann[0::2])}
+    out = capi.Sam()
+    summ = np.zeros((len(aligners), 3, 3))
+    rows = []
+    n_all = len(aligners) * world
+    per_batch = min(DUMP_READS_PER_BATCH, (DUMP_BYTES // n_all - 9 * 8 - 256) // (8 * 8))  # 8 float64 per sampled read; streams.npy: 9 per batch + header
+    for b, al in enumerate(aligners):
+        s.ck(s.lib.ssq_aligner_fetch(al, C.byref(out)), "ssq_aligner_fetch")
+        txt = [C.string_at(out.text[k], out.len[k]) for k in range(3)]
+        n = batches[b].n
+        ro = np.ctypeslib.as_array((C.c_uint64 * (n + 1)).from_address(out.read_off)).copy()
+        for k in range(3):
+            summ[b, k] = (len(txt[k]), txt[k].count(b"\n"), zlib.crc32(txt[k]))
+        for i in np.sort(np.random.default_rng(1000 + b).choice(n, min(n, per_batch), replace=False)):
+            seg = txt[0][ro[i]:ro[i + 1]]
+            f = seg.split(b"\n", 1)[0].split(b"\t")
+            if len(f) < 9:
+                rows.append((b, i, -1, -1, -1, -1, 0, zlib.crc32(seg)))
+            else:
+                rows.append((b, i, int(f[1]), cid.get(f[2].decode(), -1), int(f[3]), int(f[4]), int(f[8]), zlib.crc32(seg)))
+    sfx = "_rank%d" % rank if rank else ""
+    np.save(os.path.join(d, "streams%s.npy" % sfx), summ)
+    np.save(os.path.join(d, "main_sample%s.npy" % sfx), np.array(rows, np.float64).reshape(-1, 8))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--reads", type=int, default=10_000_000)
-    ap.add_argument("--batch", type=int, default=2_000_000)
+    ap.add_argument("--reads", type=int, default=3_000_000)
+    ap.add_argument("--batch", type=int, default=1_000_000)
     ap.add_argument("--genome-len", type=int, default=int(os.environ.get("SSQ_BENCH_GENOME", GENOME_LEN)))
-    ap.add_argument("--cache", default=os.environ.get("SSQ_BENCH_CACHE", os.path.join(ROOT, "data_cache")))
+    ap.add_argument("--cache", default=os.environ.get("SSQ_BENCH_CACHE"),
+                    help="where the synthetic genome and its index are kept between runs (default: a temporary directory removed at exit)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step computed to DIR/*.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-sample", type=int, default=0, help="reads in the CPU-arm sample (0: sized for ~15 s)")
     ap.add_argument("--streams", type=int, default=int(os.environ.get("SSQ_BENCH_STREAMS", "5")), help="host threads / CUDA streams that drive batches concurrently")
@@ -252,6 +307,11 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
+    if a.cache is None:  # one directory per run, shared by its ranks (torchrun gives them one run id); local rank 0 removes it at exit
+        a.cache = os.path.join(tempfile.gettempdir(), "ssq_bench_%d_%s" % (os.getuid(), os.environ.get("TORCHELASTIC_RUN_ID") if world > 1 else os.getpid()))
+        if local == 0:
+            import atexit
+            atexit.register(shutil.rmtree, a.cache, True)
     ncores = usable_cores()
     nb = max(1, a.reads // a.batch)
     workload = "%dM synthetic 2x%dbp PE reads (10%% duplicate pairs, 1%% chimeric) vs synthetic %d bp reference (8 contigs, planted repeats), full `bwa mem | samblaster` path: align + pair + CIGAR + dup-mark + discordant/splitter streams + SAM text" % (nb * a.batch // 1_000_000, READ_LEN, a.genome_len)
@@ -387,6 +447,8 @@ def main():
     barrier()
     ms_total = span_ms(ev)
     clocks = clk.stop()
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, s, aligners, batches, fa, rank, world)
     # ---- per-stage statistics: one extra step, batches one after the other so that stage durations are not stretched by overlap ----
     STAGES = ["upload", "seed_chain_extend", "sort_dedup_patch", "insert_size_stats", "mate_rescue", "pair_mapq_plan", "cigar_nm_md", "samblaster_dupset", "sam_text", "fetch",
               "k_smem", "k_sa", "k_chain", "k_extend", "k_select"]
@@ -440,6 +502,9 @@ def main():
         ee[k][1].record(exts[k])
     barrier()
     ms_e2e = span_ms(ee)
+    mem_in_use = (lambda f: (f[1] - f[0]) / 1e9)(torch.cuda.mem_get_info(local))  # all processes on the device
+    for al in aligners:  # the parity check below needs an aligner of its own
+        s.aligner_free(al)
     h2d = sum(bt.h2d for bt in batches)
     tmax = torch.tensor([ms_total, ms_e2e], device="cuda", dtype=torch.float64)
     if world > 1:
@@ -448,13 +513,11 @@ def main():
     value = world * n_reads_step * a.steps / (ms_total / 1000.0)
     e2e_v = world * n_reads_step * a.steps / (ms_e2e / 1000.0)
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = HBM_GBPS
+        peak_src = "H100 SXM data sheet (HBM3), not measured"
+        n_sm = torch.cuda.get_device_properties(local).multi_processor_count
+        ghz = (clocks["sm_max_mhz"] or 1980) / 1000.0  # 1980 MHz: the H100 SXM boost clock when nvidia-smi cannot say
+        alu_peak = n_sm * 128 * ghz  # G lane-operations/s: 128 integer lanes per SM
         blk = float(L.ssq_index_info(idx, 7))
         st = dict(zip(STAGES, (stage_ms / nb).tolist()))
         fq_bytes = sum(bt.h2d for bt in batches) / nb
@@ -464,9 +527,9 @@ def main():
             "k_sa (SA look-up)": {"ms": st["k_sa"], "bytes": (blk * counters[1] + float(L.ssq_index_info(idx, 8)) * counters[2]) / nb},
             "k_chain": {"ms": st["k_chain"], "bytes": None},
             "k_extend (ksw_extend2)": {"ms": st["k_extend"], "bytes": counters[5] / nb, "gcups": counters[4] / nb / (st["k_extend"] * 1e6) if st["k_extend"] else None,
-                                       # ALU roofline: ~16 integer lane-operations per DP cell (SASS of k_ext_run's inner loop) against 148 SMs x 128 lanes x clock
+                                       # ALU roofline: ~16 integer lane-operations per DP cell (SASS of k_ext_run's inner loop) against SMs x 128 lanes x max clock
                                        "roofline": {"bound": "alu", "unit": "G lane-ops/s", "ops_per_cell": 16, "achieved": 16 * counters[4] / nb / (st["k_extend"] * 1e6) if st["k_extend"] else None,
-                                                    "peak": 148 * 128 * 1.965, "frac": (16 * counters[4] / nb / (st["k_extend"] * 1e6)) / (148 * 128 * 1.965) if st["k_extend"] else None}},
+                                                    "peak": alu_peak, "frac": (16 * counters[4] / nb / (st["k_extend"] * 1e6)) / alu_peak if st["k_extend"] else None}},
             "k_select": {"ms": st["k_select"], "bytes": None},
             "k_dedup (sort/dedup/patch)": {"ms": st["sort_dedup_patch"], "bytes": None},
             "k_pestat + host reduction": {"ms": st["insert_size_stats"], "bytes": None},
@@ -483,23 +546,7 @@ def main():
         # the single dominant kernel: the backward sweeps of the seeding when the split seeding ran (their own events / block counter), else the stage
         cand = [k for k in kern if kern[k]["bytes"] is not None and not (k == "k_smem (seeding, all passes)" and bwd_us)]
         dom = max(cand, key=lambda k: kern[k]["ms"])
-        traffic = None
-        try:  # DRAM bytes of the same kernel from the committed `ncu --set full` capture (same batch size and reference)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-            if dom in tj and a.batch == tj["batch_reads"] and a.genome_len == tj["genome_bp"]:
-                traffic = tj[dom]["dram_bytes_read"] + tj[dom]["dram_bytes_write"]
-        except Exception:
-            pass
         ach = kern[dom]["achieved_GBps"] or 0.0
-        rnd = None
-        try:  # what this device serves when the reads are dependent random 32-byte sectors over a table of the rank structure's size (measured, profiles/)
-            rj = json.load(open(os.path.join(ROOT, "profiles", "r02_random_sector.json")))
-            tab_gb = a.genome_len * 2 * 32 / 64 / 2**30  # 32 bytes per 64 BWT symbols, both strands
-            key = min(rj["table_GB"], key=lambda k: abs(float(k) - tab_gb))
-            if "k_smem" in dom and abs(float(key) - tab_gb) < 0.25 * tab_gb:
-                rnd = {"GBps": rj["table_GB"][key], "table_GB": float(key), "frac_of_ceiling": ach / rj["table_GB"][key], "source": "profiles/r02_random_sector.log (tools/random_sector_bench.cu)"}
-        except Exception:
-            pass
         res = {"metric": metric, "value": value, "unit": "reads/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_total / a.steps,
                "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "int32", "data": "synthetic",
                "config": {"workload": workload, "batch_reads": a.batch, "batches_per_step": nb, "streams": nstreams, "genome_bp": a.genome_len,
@@ -509,9 +556,11 @@ def main():
                           "samblaster": " ".join(SB_ARGS)},
                "clocks": clocks, "gpu_launches": int(counters[6]) * a.steps + 16 * nb * a.steps,  # seed..extend launches counted by the library + the 16 pipeline kernels of a batch (k_dedup .. k_text; CUB scans / sorts not counted)
                "e2e": {"value": e2e_v, "unit": "reads/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h_step[0], "ms_per_step": ms_e2e / a.steps},
-               "roofline": {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+               "device": {"name": torch.cuda.get_device_name(local), "sms": n_sm, "power_limit_w": clocks.get("power_limit_w"),
+                          "device_mem_in_use_GB": mem_in_use},
+               "roofline": {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                             "peak_source": peak_src, "algorithmic_bytes_per_launch": kern[dom]["bytes"], "launch_ms": kern[dom]["ms"], "rank_block_bytes": blk,
-                            "access_pattern": "dependent random 32-byte sector reads (one or two rank blocks per FM-index extension)", "random_sector_ceiling": rnd},
+                            "access_pattern": "dependent random 32-byte sector reads (one or two rank blocks per FM-index extension)"},
                "kernels": kern,
                "work_per_step": {"occ_blocks_smem": counters[0], "occ_blocks_sa": counters[1], "sa_samples": counters[2], "sw_calls": counters[3], "sw_cells": counters[4], "seeds": counters[7],
                                  "alignments_written": n_tasks, "sam_bytes": text_bytes, "pairs_through_mate_rescue": n_rescue, "alignments_with_banded_dp": n_gapped, "rescue_sw_passes": n_swl, "rescue_sw_cells": swl_cells},
@@ -539,8 +588,6 @@ def main():
                 print(json.dumps(res))
                 raise SystemExit("bench.py: GPU output differs from the oracle on the CPU-baseline sample")
         print(json.dumps(res))
-    for al in aligners:
-        s.aligner_free(al)
     if comm is not None:
         L.ssq_comm_free(comm)
     else:

@@ -1,9 +1,9 @@
 /*
- * ssq.h — C-ABI of libssq.so, the B200-native implementation of the `speedseq align` hot path.
+ * ssq.h — C-ABI of libssq.so, the H100-native (sm_90a) implementation of the `speedseq align` hot path.
  *
  * The reference's drop-in boundary for this path is a PROCESS boundary, not an FFI:
- * bin/speedseq sources speedseq.config (/root/reference/bin/speedseq:15-24,361) and interpolates
- * $BWA and $SAMBLASTER into the pipeline text at /root/reference/bin/speedseq:437-449 (interleaved)
+ * bin/speedseq sources speedseq.config (speedseq/bin/speedseq:15-24,361) and interpolates
+ * $BWA and $SAMBLASTER into the pipeline text at speedseq/bin/speedseq:437-449 (interleaved)
  * and :467-479 (two files); the index is made by `$BWA index` at :389.  libssq.so is what the two
  * replacement executables (speedseq_b200/bin/bwa, speedseq_b200/bin/samblaster) link; its entry
  * points are the batch forms of the functions those tools spend their time in (SURVEY.md §8a).
@@ -12,7 +12,7 @@
  *
  * Conventions: plain pointers and sizes, caller-owned HOST buffers unless a name ends in _dev,
  * int return code (0 = ok, <0 = SSQ_E*), no global state other than the CUDA context, one CUDA
- * stream per handle.  Every entry point fails with SSQ_ENOGPU when no sm_100 device is usable —
+ * stream per handle.  Every entry point fails with SSQ_ENOGPU when no sm_90 (H100) device is usable —
  * there is no CPU fallback inside this library.
  */
 #ifndef SSQ_H
@@ -41,7 +41,7 @@ int ssq_device_count(void);
 
 /* ---------------------------------------------------------------- options ----
  * Scoring/heuristic parameters of `bwa mem`; speedseq passes none of them on the command line
- * (/root/reference/bin/speedseq:438), so ssq_opts_default() is what the pipeline runs with.
+ * (speedseq/bin/speedseq:438), so ssq_opts_default() is what the pipeline runs with.
  * Replaces upstream mem_opt_init(). */
 typedef struct {
 	int32_t a, b, o_del, e_del, o_ins, e_ins;
@@ -56,11 +56,11 @@ void ssq_opts_default(ssq_opts_t *o);
 
 /* ------------------------------------------------------------------ index ----
  * Device-resident FM index + packed reference.  ssq_index_load replaces upstream bwa_idx_load()
- * (start of `$BWA mem`, /root/reference/bin/speedseq:438): reads PREFIX.{bwt,sa,pac,ann,amb} in the
- * on-disk format of the reference's goldens (/root/reference/example/data/ *.fasta.{amb,ann,pac,bwt,sa})
+ * (start of `$BWA mem`, speedseq/bin/speedseq:438): reads PREFIX.{bwt,sa,pac,ann,amb} in the
+ * on-disk format of the reference's goldens (speedseq/example/data/ *.fasta.{amb,ann,pac,bwt,sa})
  * and uploads them to `device`. */
 typedef struct ssq_index ssq_index_t;
-/* `$BWA index $REF` (/root/reference/bin/speedseq:389): FASTA (plain or gz) -> PREFIX.{amb,ann,pac,bwt,sa}, byte-identical
+/* `$BWA index $REF` (speedseq/bin/speedseq:389): FASTA (plain or gz) -> PREFIX.{amb,ann,pac,bwt,sa}, byte-identical
  * to the reference's goldens for example/data; suffix sorting, BWT, occ checkpoints and SA sampling run on `device`.
  * References beyond the device sort's 2^31 - 2 suffixes (1.07 Gbp; a whole human genome has 6.2 G) are indexed on the host
  * instead — induced sorting with 5-byte entries, same files, no GPU touched (about 15 bytes of host memory per base pair:
@@ -179,7 +179,7 @@ int ssq_mem_batch_sam(const ssq_index_t *idx, const ssq_opts_t *opt, int n_reads
 void ssq_free(void *p);
 
 /* ----------------------------------------- `bwa mem | samblaster`, HBM-resident ----
- * The whole pipe of /root/reference/bin/speedseq:438-439 (interleaved) / :468-469 (two files) for one batch of reads:
+ * The whole pipe of speedseq/bin/speedseq:438-439 (interleaved) / :468-469 (two files) for one batch of reads:
  * `$BWA mem -t T [-p] [-C] [-I ..] -R RG REF FQ.. | $SAMBLASTER [--excludeDups] --addMateTags --maxSplitCount C
  * --minNonOverlap M --splitterFile F --discordantFile F`.  Reads go in as the FASTQ fields (concatenated, with offsets), the three
  * SAM record streams come out (main, splitters, discordants; headers are the caller's business: they depend on argv).  Between
@@ -224,7 +224,7 @@ int ssq_aligner_run(ssq_aligner_t *al, const ssq_reads_t *reads, const ssq_pesta
 int ssq_aligner_upload(ssq_aligner_t *al, const ssq_reads_t *reads);
 int ssq_aligner_compute(ssq_aligner_t *al, const ssq_pestat_t *pes0, int verbose);
 /* FASTQ ingest on the device instead of ssq_aligner_upload (upstream bseq_read -> kseq_read inside `$BWA mem`, speedseq:438,468;
- * tokenisation rules of /root/reference/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231).  fq1 / fq2: raw, uncompressed text of
+ * tokenisation rules of speedseq/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231).  fq1 / fq2: raw, uncompressed text of
  * the FASTQ input(s) from a record boundary on (fq2 == NULL: one file; interleaved: adjacent records are mates, `-p`); final: no
  * more text follows.  The device finds the records, closes the batch where bwa would (bases >= chunk_bases and an even number of
  * reads), strips /1 /2, and packs names, bases, qualities and (keep_comment, `-C`) comments into the aligner's batch buffers;

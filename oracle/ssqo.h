@@ -5,15 +5,15 @@
  * link or execute anything under oracle/.  The product (speedseq_b200/) never does.
  *
  * What it restates: the arithmetic behind `$BWA mem` and `$SAMBLASTER` as called at
- * /root/reference/bin/speedseq:438-439,468-469 (and `$BWA index` at :389).  Those two tools are
+ * speedseq/bin/speedseq:438-439,468-469 (and `$BWA index` at :389).  Those two tools are
  * un-vendored submodules in the reference checkout (src/bwa, src/samblaster are EMPTY; pins in
- * /root/reference/.SUBMODULES.json:23-29,51-57 = lh3/bwa@d82444c1, GregoryFaust/samblaster@b6426391),
+ * speedseq/.SUBMODULES.json:23-29,51-57 = lh3/bwa@d82444c1, GregoryFaust/samblaster@b6426391),
  * so this file set restates their *published* algorithms (BWA-MEM 0.7.12-series behaviour,
  * samblaster 0.1.2x behaviour; SURVEY.md Appendix A/B) in plain scalar C.
  *
  * PARITY STATUS
  *   - index build/load (.amb .ann .pac .bwt .sa): PINNED by the reference's own golden files
- *     /root/reference/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa}
+ *     speedseq/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa}
  *     (tests/test_oracle_index.py rebuilds them byte-for-byte; a copy of the goldens' sha256 and a
  *     small derived fixture live under tests/golden/).
  *   - alignment records / dup flags / discordant+splitter sets: **parity unpinned** — the reference

@@ -1,7 +1,7 @@
 /*
  * ssqo_bwt.c — ORACLE (test infrastructure): FM-index occ / bidirectional extension / SMEM search /
  * SA lookup.  SURVEY.md §8a rows a4, a5; called from inside `$BWA mem`
- * (/root/reference/bin/speedseq:438,468).  Upstream names (not in tree): bwt_occ4, bwt_2occ4,
+ * (speedseq/bin/speedseq:438,468).  Upstream names (not in tree): bwt_occ4, bwt_2occ4,
  * bwt_extend, bwt_smem1a, bwt_seed_strategy1, bwt_invPsi, bwt_sa.  Layout of the occ-interleaved
  * BWT is the one verified against the reference goldens (SURVEY.md §8c).
  */

@@ -1,9 +1,9 @@
 /*
  * ssqo_index.c — ORACLE (test infrastructure): `bwa index` restatement and index loader.
  *
- * Follows: call site /root/reference/bin/speedseq:386-391 (`$BWA index $REF` must create
+ * Follows: call site speedseq/bin/speedseq:386-391 (`$BWA index $REF` must create
  * REF.{amb,ann,pac,bwt,sa}); on-disk format verified against the goldens
- * /root/reference/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa}
+ * speedseq/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa}
  * (SURVEY.md §8c "Verified on-disk index format").  Upstream names (not in tree): bns_fasta2bntseq,
  * bwt_pac2bwt, bwt_bwtupdate_core, bwt_cal_sa, bwa_idx_load.
  */

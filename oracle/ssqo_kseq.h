@@ -1,6 +1,6 @@
 /*
  * ssqo_kseq.h — ORACLE (test infrastructure): FASTA/FASTQ tokeniser with the semantics of the
- * reference's in-tree parser /root/reference/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231
+ * reference's in-tree parser speedseq/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231
  * (name = up to first whitespace, comment = rest of header line, multi-line sequence, '+' line,
  * quality read until it is at least as long as the sequence).  gz input through zlib.
  */

@@ -4,7 +4,7 @@
  * z-drop), a14 (ksw_global2, banded global DP + traceback), a11 (ksw_align2 = Farrar-striped local
  * SW, u8 then i16 — restated here as a scalar emulation of the striped evaluation order, including
  * its lane/segment artefacts, so that scores, end points and the 2nd-best score agree).
- * Call sites in the reference: inside `$BWA mem`, /root/reference/bin/speedseq:438,468.
+ * Call sites in the reference: inside `$BWA mem`, speedseq/bin/speedseq:438,468.
  */
 #include <stdlib.h>
 #include <string.h>

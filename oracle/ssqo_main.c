@@ -1,5 +1,5 @@
 /* ssqo_main.c — ORACLE (test infrastructure): CLI with the argv contract of the reference's
- * `$BWA index|mem` and `$SAMBLASTER` call sites (/root/reference/bin/speedseq:389,438-439). */
+ * `$BWA index|mem` and `$SAMBLASTER` call sites (speedseq/bin/speedseq:389,438-439). */
 #include <string.h>
 #include <stdio.h>
 #include "ssqo.h"

@@ -2,7 +2,7 @@
  * ssqo_mem.c — ORACLE (test infrastructure): single-end core of BWA-MEM.
  * SURVEY.md §8a rows a4-a9, a13-a15: seeding passes, chaining, chain filter, seed extension,
  * de-duplication/patching, primary marking, MAPQ, CIGAR/NM/MD and SAM text.
- * Reference call site: `$BWA mem -t T [-p] -R RG REF FQ` at /root/reference/bin/speedseq:438,468
+ * Reference call site: `$BWA mem -t T [-p] -R RG REF FQ` at speedseq/bin/speedseq:438,468
  * (every scoring option at its default).  Upstream names (not in tree): mem_collect_intv,
  * mem_chain, mem_chain_flt, mem_chain2aln, mem_sort_dedup_patch, mem_patch_reg,
  * mem_mark_primary_se, mem_approx_mapq_se, bwa_gen_cigar2, mem_reg2aln, mem_aln2sam, mem_gen_alt.

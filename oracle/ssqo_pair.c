@@ -2,7 +2,7 @@
  * ssqo_pair.c — ORACLE (test infrastructure): paired-end half of BWA-MEM and the `bwa mem` driver.
  * SURVEY.md §8a rows a3 (batching), a10 (insert-size statistics per batch), a11 (mate rescue),
  * a12 (pairing), a13 (paired MAPQ), a15 (SAM text + header).
- * Reference call site: /root/reference/bin/speedseq:438 (`-p` interleaved) and :468 (two files).
+ * Reference call site: speedseq/bin/speedseq:438 (`-p` interleaved) and :468 (two files).
  * Upstream names (not in tree): mem_pestat, mem_matesw, mem_pair, mem_sam_pe, mem_process_seqs,
  * bseq_read, bseq_classify, main_mem, bwa_set_rg, bwa_print_sam_hdr.
  */

@@ -1,5 +1,5 @@
 /* ssqo_par.h — ORACLE (test infrastructure): minimal pthread parallel-for (dynamic chunks of 16),
- * the stand-in for bwa's kt_for worker pool (`bwa mem -t N`, /root/reference/bin/speedseq:438). */
+ * the stand-in for bwa's kt_for worker pool (`bwa mem -t N`, speedseq/bin/speedseq:438). */
 #ifndef SSQO_PAR_H
 #define SSQO_PAR_H
 #include <pthread.h>

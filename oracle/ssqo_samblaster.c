@@ -2,7 +2,7 @@
  * ssqo_samblaster.c — ORACLE (test infrastructure): SAMBLASTER restatement.
  * SURVEY.md §8a rows a16-a19 and Appendix B.  Reference call site:
  *   $SAMBLASTER [--excludeDups] --addMateTags --maxSplitCount C --minNonOverlap M
- *               --splitterFile FIFO --discordantFile FIFO      (/root/reference/bin/speedseq:439,469)
+ *               --splitterFile FIFO --discordantFile FIFO      (speedseq/bin/speedseq:439,469)
  * stdin = name-grouped SAM from `bwa mem`, stdout = SAM with 0x400 set on duplicates (first-seen pair
  * per signature is kept), MC/MQ appended, side streams = discordant pairs and split reads.
  * The signature of a pair is (contig, 5'-unclipped position, strand) of both primary lines, ends

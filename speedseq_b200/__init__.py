@@ -1,4 +1,4 @@
-"""speedseq_b200 — B200-native `speedseq align` hot path (BWA-MEM seed/chain/extend + SAMBLASTER dup-marking).
+"""speedseq_b200 — H100-native (sm_90a) `speedseq align` hot path (BWA-MEM seed/chain/extend + SAMBLASTER dup-marking).
 
 The product is the C-ABI library speedseq_b200/libssq.so (include/ssq.h) and the two CLI shims under speedseq_b200/bin
 that plug into the reference's speedseq.config (BWA=, SAMBLASTER=).  This Python package only locates the library;

@@ -1,13 +1,13 @@
 /*
- * bwa — drop-in for the `$BWA` entry of speedseq.config (/root/reference/bin/speedseq.config:13), a thin C shim over
+ * bwa — drop-in for the `$BWA` entry of speedseq.config (speedseq/bin/speedseq.config:13), a thin C shim over
  * libssq.so.  Honours the argv/stdio contract of the reference's call sites:
- *     $BWA index REF                                              /root/reference/bin/speedseq:389
+ *     $BWA index REF                                              speedseq/bin/speedseq:389
  *     $BWA mem -t T [-p] [-C] [-I f[,f[,i[,i]]]] -R '@RG\tID:..' REF FQ1 [FQ2]   speedseq:438,468,1961
  * stdout = SAM (header, then records name-grouped in input order).  All base-level work AND the SAM text come from the GPU
  * (ssq_index_build, ssq_aligner_run: include/ssq.h); this file parses argv, tokenises FASTQ straight into the concatenated
  * layout the aligner takes, forms batches the way the reference's `bwa mem` does (bases >= 10 M x T and an even read count), and
  * writes what comes back.
- * FASTQ tokenisation follows the reference's in-tree parser /root/reference/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231.
+ * FASTQ tokenisation follows the reference's in-tree parser speedseq/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231.
  *
  * Fused mode.  speedseq pipes `$BWA mem | $SAMBLASTER ...` (speedseq:438-439).  When the environment variable
  * SSQ_FUSE_SAMBLASTER holds samblaster's option string (speedseq.config can export it from speedseq's own variables, see
@@ -482,7 +482,7 @@ static int main_index(int argc, char **argv)
 
 int main(int argc, char **argv)
 {
-	if (argc < 2) { fprintf(stderr, "Usage: bwa <index|mem> [options]   (B200-native shim over libssq, behaviour of bwa %s)\n", SHIM_VERSION); return 1; }
+	if (argc < 2) { fprintf(stderr, "Usage: bwa <index|mem> [options]   (H100 shim over libssq, behaviour of bwa %s)\n", SHIM_VERSION); return 1; }
 	if (!strcmp(argv[1], "index")) return main_index(argc - 1, argv + 1);
 	if (!strcmp(argv[1], "mem")) return main_mem(argc - 1, argv + 1, argv[0]);
 	fprintf(stderr, "[main] unrecognized command '%s'\n", argv[1]);

@@ -1,6 +1,6 @@
 /* sambamba_main.c — the `sambamba` the pipeline's align step can be pointed at (speedseq.config `SAMBAMBA=`) when the `bwa` /
  * `samblaster` shims run in BAM mode (SSQ_FUSE_BAM, see ssq_fuse.h): the main records then arrive as coordinate-sorted runs of BAM
- * records made on the device instead of SAM text, and the two calls of /root/reference/bin/speedseq:440-441
+ * records made on the device instead of SAM text, and the two calls of speedseq/bin/speedseq:440-441
  *     $SAMBAMBA view -S -f bam -l 0 /dev/stdin | $SAMBAMBA sort -t T -m M --tmpdir=D -o out.bam /dev/stdin
  * become a pass-through and a merge of sorted runs:
  *   view : stdin that carries the run marker is copied to stdout unchanged;
@@ -36,7 +36,7 @@ static const char *real_path(void)
 }
 static void need_real(const char *why)
 {
-	fprintf(stderr, "sambamba (B200 shim): %s needs the real sambamba: set SSQ_SAMBAMBA_REAL to its path (or install it as `sambamba.real` next to %s)\n", why, g_self);
+	fprintf(stderr, "sambamba (GPU shim): %s needs the real sambamba: set SSQ_SAMBAMBA_REAL to its path (or install it as `sambamba.real` next to %s)\n", why, g_self);
 	exit(1);
 }
 static void exec_real(char **argv, const char *why)
@@ -44,7 +44,7 @@ static void exec_real(char **argv, const char *why)
 	const char *r = real_path();
 	if (!r) need_real(why);
 	execv(r, argv);
-	fprintf(stderr, "sambamba (B200 shim): cannot execute %s: %s\n", r, strerror(errno));
+	fprintf(stderr, "sambamba (GPU shim): cannot execute %s: %s\n", r, strerror(errno));
 	exit(1);
 }
 static int write_all(int fd, const void *p, size_t n)
@@ -64,7 +64,7 @@ static int feed_real(char **argv, const char *head, size_t n_head, const char *w
 	if (pipe(fd)) { perror("pipe"); return 1; }
 	pid = fork();
 	if (pid < 0) { perror("fork"); return 1; }
-	if (pid == 0) { dup2(fd[0], 0); close(fd[0]); close(fd[1]); execv(r, argv); fprintf(stderr, "sambamba (B200 shim): cannot execute %s: %s\n", r, strerror(errno)); _exit(127); }
+	if (pid == 0) { dup2(fd[0], 0); close(fd[0]); close(fd[1]); execv(r, argv); fprintf(stderr, "sambamba (GPU shim): cannot execute %s: %s\n", r, strerror(errno)); _exit(127); }
 	close(fd[0]);
 	signal(SIGPIPE, SIG_IGN);
 	if (write_all(fd[1], head, n_head) == 0) for (;;) { ssize_t n = read(0, buf, sizeof buf); if (n < 0 && errno == EINTR) continue; if (n <= 0) break; if (write_all(fd[1], buf, (size_t)n)) break; }
@@ -111,7 +111,7 @@ static const uint8_t *src_peek(src_t *s, size_t *rec_len)
 	if (!s->fp) {
 		if (s->at + 4 > s->len) return 0;
 		memcpy(&bs, s->mem + s->at, 4);
-		if (bs < 32 || s->at + 4 + (size_t)bs > s->len) { fprintf(stderr, "sambamba (B200 shim): a run is not a sequence of BAM records\n"); exit(1); }
+		if (bs < 32 || s->at + 4 + (size_t)bs > s->len) { fprintf(stderr, "sambamba (GPU shim): a run is not a sequence of BAM records\n"); exit(1); }
 		*rec_len = 4 + (size_t)bs;
 		return s->mem + s->at;
 	}
@@ -121,7 +121,7 @@ static const uint8_t *src_peek(src_t *s, size_t *rec_len)
 		if (have >= 4) { memcpy(&bs, s->buf + s->pos, 4); want = 4 + (size_t)bs; if (have >= want) { *rec_len = want; return s->buf + s->pos; } }
 		if (s->pos) { memmove(s->buf, s->buf + s->pos, have); s->fill = have; s->pos = 0; }
 		if (want > s->cap) { s->cap = want * 2; s->buf = (uint8_t*)realloc(s->buf, s->cap); }
-		{ const size_t n = fread(s->buf + s->fill, 1, s->cap - s->fill, s->fp); if (!n) { if (have) { fprintf(stderr, "sambamba (B200 shim): truncated spill file\n"); exit(1); } return 0; } s->fill += n; }
+		{ const size_t n = fread(s->buf + s->fill, 1, s->cap - s->fill, s->fp); if (!n) { if (have) { fprintf(stderr, "sambamba (GPU shim): truncated spill file\n"); exit(1); } return 0; } s->fill += n; }
 	}
 }
 static void src_advance(src_t *s, size_t rec_len) { if (s->fp) s->pos += rec_len; else s->at += rec_len; }
@@ -176,8 +176,8 @@ static void *flush_main(void *a) /* one buffer: compressed in slices on `threads
 	job_main(&jobs[0]);
 	for (k = 1; k < nj; ++k) pthread_join(th[k], 0);
 	for (k = 0; k < nj; ++k) {
-		if (jobs[k].rc) { fprintf(stderr, "sambamba (B200 shim): BGZF compression failed: %s\n", ssq_last_error()); exit(1); }
-		if (fwrite(jobs[k].out, 1, jobs[k].out_len, f->fp) != jobs[k].out_len) { perror("sambamba (B200 shim): write"); exit(1); }
+		if (jobs[k].rc) { fprintf(stderr, "sambamba (GPU shim): BGZF compression failed: %s\n", ssq_last_error()); exit(1); }
+		if (fwrite(jobs[k].out, 1, jobs[k].out_len, f->fp) != jobs[k].out_len) { perror("sambamba (GPU shim): write"); exit(1); }
 		ssq_free(jobs[k].out);
 	}
 	return 0;
@@ -204,7 +204,7 @@ static void bgzf_put(void *ctx, const uint8_t *p, size_t n)
 		if (o->n == o->cap) bgzf_flush(o);
 	}
 }
-static void file_put(void *ctx, const uint8_t *p, size_t n) { if (fwrite(p, 1, n, (FILE*)ctx) != n) { perror("sambamba (B200 shim): spill write"); exit(1); } }
+static void file_put(void *ctx, const uint8_t *p, size_t n) { if (fwrite(p, 1, n, (FILE*)ctx) != n) { perror("sambamba (GPU shim): spill write"); exit(1); } }
 
 static size_t parse_mem(const char *s)
 {
@@ -232,14 +232,14 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 		size_t got = 0;
 		while (h->n - at < sizeof fh && head_more(h)) {}
 		if (h->n - at == 0) break;
-		if (h->n - at < sizeof fh) { fprintf(stderr, "sambamba (B200 shim): truncated run stream\n"); return 1; }
+		if (h->n - at < sizeof fh) { fprintf(stderr, "sambamba (GPU shim): truncated run stream\n"); return 1; }
 		memcpy(&fh, h->p + at, sizeof fh); at += sizeof fh;
-		if (memcmp(fh.magic, SSQ_FRAME_MAGIC, 8) != 0 || fh.stream != SSQ_STREAM_BAM_RUN) { fprintf(stderr, "sambamba (B200 shim): corrupt run stream\n"); return 1; }
+		if (memcmp(fh.magic, SSQ_FRAME_MAGIC, 8) != 0 || fh.stream != SSQ_STREAM_BAM_RUN) { fprintf(stderr, "sambamba (GPU shim): corrupt run stream\n"); return 1; }
 		run = (uint8_t*)malloc(fh.len ? fh.len : 1);
-		if (!run) { fprintf(stderr, "sambamba (B200 shim): out of memory\n"); return 1; }
+		if (!run) { fprintf(stderr, "sambamba (GPU shim): out of memory\n"); return 1; }
 		{ const size_t k = h->n - at < fh.len ? h->n - at : (size_t)fh.len; memcpy(run, h->p + at, k); at += k; got = k; }
 		if (at == h->n) { h->n = 0; at = 0; } /* the look-ahead buffer is used up: read straight into the run */
-		while (got < fh.len) { ssize_t n = read(0, run + got, fh.len - got); if (n < 0 && errno == EINTR) continue; if (n <= 0) { fprintf(stderr, "sambamba (B200 shim): truncated run stream\n"); return 1; } got += (size_t)n; }
+		while (got < fh.len) { ssize_t n = read(0, run + got, fh.len - got); if (n < 0 && errno == EINTR) continue; if (n <= 0) { fprintf(stderr, "sambamba (GPU shim): truncated run stream\n"); return 1; } got += (size_t)n; }
 		if (n_mem == m_mem) { m_mem = m_mem ? m_mem * 2 : 64; mem = (src_t*)realloc(mem, sizeof(src_t) * (size_t)m_mem); }
 		memset(&mem[n_mem], 0, sizeof(src_t)); mem[n_mem].mem = run; mem[n_mem].len = fh.len; ++n_mem; in_mem += fh.len;
 		if (in_mem > mem_limit) { /* merge what is held and spill it */
@@ -247,9 +247,9 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 			FILE *fp;
 			mkdir(tmpdir, 0777); /* sambamba creates its --tmpdir too */
 			snprintf(fn, sizeof fn, "%s/ssq_sort_%ld_%d.run", tmpdir, (long)getpid(), n_spill);
-			if (!(fp = fopen(fn, "wb"))) { fprintf(stderr, "sambamba (B200 shim): cannot create %s: %s\n", fn, strerror(errno)); return 1; }
+			if (!(fp = fopen(fn, "wb"))) { fprintf(stderr, "sambamba (GPU shim): cannot create %s: %s\n", fn, strerror(errno)); return 1; }
 			merge_sources(mem, n_mem, file_put, fp);
-			if (fclose(fp)) { perror("sambamba (B200 shim): spill"); return 1; }
+			if (fclose(fp)) { perror("sambamba (GPU shim): spill"); return 1; }
 			for (i = 0; i < n_mem; ++i) free((void*)mem[i].mem);
 			n_mem = 0; in_mem = 0;
 			if (n_spill == m_spill) { m_spill = m_spill ? m_spill * 2 : 16; spill_fn = (char**)realloc(spill_fn, sizeof(char*) * (size_t)m_spill); }
@@ -262,10 +262,10 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 	for (i = 0; i < n_mem; ++i) spill[n_spill + i] = mem[i];
 	/* output: header block(s), records, end-of-file block */
 	memset(&o, 0, sizeof o);
-	if (!(o.fp = fopen(out_fn, "wb"))) { fprintf(stderr, "sambamba (B200 shim): cannot create %s: %s\n", out_fn, strerror(errno)); return 1; }
+	if (!(o.fp = fopen(out_fn, "wb"))) { fprintf(stderr, "sambamba (GPU shim): cannot create %s: %s\n", out_fn, strerror(errno)); return 1; }
 	o.threads = threads < 1 ? 1 : threads > 64 ? 64 : threads; o.level = level; o.cap = (size_t)0xff00 * 256 * (size_t)o.threads; o.buf = (uint8_t*)malloc(o.cap); o.alt = (uint8_t*)malloc(o.cap);
-	if (!o.buf || !o.alt) { fprintf(stderr, "sambamba (B200 shim): out of memory\n"); return 1; }
-	if (ssq_bam_header_text(hdr_text, 1, &hdr_sorted)) { fprintf(stderr, "sambamba (B200 shim): %s\n", ssq_last_error()); return 1; }
+	if (!o.buf || !o.alt) { fprintf(stderr, "sambamba (GPU shim): out of memory\n"); return 1; }
+	if (ssq_bam_header_text(hdr_text, 1, &hdr_sorted)) { fprintf(stderr, "sambamba (GPU shim): %s\n", ssq_last_error()); return 1; }
 	{ /* "BAM\1", text, reference table from the @SQ lines */
 		const uint32_t l_text = (uint32_t)strlen(hdr_sorted);
 		uint32_t n_ref = 0;
@@ -277,7 +277,7 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 			const char *e = strchr(p, '\n'), *sn = 0, *ln = 0, *f;
 			char name[1024]; uint32_t l_name; int32_t l_ref;
 			for (f = p; f && f < e; f = memchr(f + 1, '\t', (size_t)(e - f - 1))) { if (!strncmp(f, "\tSN:", 4)) sn = f + 4; else if (!strncmp(f, "\tLN:", 4)) ln = f + 4; }
-			if (!sn || !ln) { fprintf(stderr, "sambamba (B200 shim): @SQ line without SN / LN\n"); return 1; }
+			if (!sn || !ln) { fprintf(stderr, "sambamba (GPU shim): @SQ line without SN / LN\n"); return 1; }
 			{ size_t k = 0; while (sn[k] != '\t' && sn[k] != '\n' && k + 1 < sizeof name) { name[k] = sn[k]; ++k; } name[k] = 0; l_name = (uint32_t)k + 1; }
 			l_ref = (int32_t)atoll(ln);
 			bgzf_put(&o, (const uint8_t*)&l_name, 4); bgzf_put(&o, (const uint8_t*)name, l_name); bgzf_put(&o, (const uint8_t*)&l_ref, 4);
@@ -287,8 +287,8 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 	merge_sources(spill, n_spill + n_mem, bgzf_put, &o);
 	bgzf_flush(&o);
 	bgzf_wait(&o);
-	{ void *eofb = 0; size_t el = 0; if (ssq_bgzf_compress("", 0, level, 1, &eofb, &el)) { fprintf(stderr, "sambamba (B200 shim): %s\n", ssq_last_error()); return 1; } fwrite(eofb, 1, el, o.fp); ssq_free(eofb); }
-	if (fclose(o.fp)) { perror("sambamba (B200 shim): close"); return 1; }
+	{ void *eofb = 0; size_t el = 0; if (ssq_bgzf_compress("", 0, level, 1, &eofb, &el)) { fprintf(stderr, "sambamba (GPU shim): %s\n", ssq_last_error()); return 1; } fwrite(eofb, 1, el, o.fp); ssq_free(eofb); }
+	if (fclose(o.fp)) { perror("sambamba (GPU shim): close"); return 1; }
 	for (i = 0; i < n_spill; ++i) { fclose(spill[i].fp); unlink(spill_fn[i]); }
 	return 0;
 }
@@ -334,7 +334,7 @@ int main(int argc, char **argv)
 		}
 		if (!in || (strcmp(in, "/dev/stdin") && strcmp(in, "-"))) exec_real(argv, "`sort` of a file");
 		if (!sniff_runs(&h, &body)) return feed_real(argv, h.p, h.n, "`sort` of ordinary BAM");
-		if (by_name || !out_fn) { fprintf(stderr, "sambamba (B200 shim): the run stream can only be coordinate-sorted into a file (-o)\n"); return 1; }
+		if (by_name || !out_fn) { fprintf(stderr, "sambamba (GPU shim): the run stream can only be coordinate-sorted into a file (-o)\n"); return 1; }
 		if (getenv("SSQ_SORT_SPILL_BYTES")) mem_limit = 2 * (size_t)atoll(getenv("SSQ_SORT_SPILL_BYTES")); /* tests: force the spill path on small inputs */
 		return sort_runs(&h, body, out_fn, threads, level, mem_limit / 2, tmpdir);
 	}

@@ -1,6 +1,6 @@
 /*
- * samblaster — drop-in for the `$SAMBLASTER` entry of speedseq.config (/root/reference/bin/speedseq.config:14), a C shim
- * over libssq.so.  Argv/stdio contract of the reference's call sites (/root/reference/bin/speedseq:439,469,1963):
+ * samblaster — drop-in for the `$SAMBLASTER` entry of speedseq.config (speedseq/bin/speedseq.config:14), a C shim
+ * over libssq.so.  Argv/stdio contract of the reference's call sites (speedseq/bin/speedseq:439,469,1963):
  *     $SAMBLASTER [--excludeDups] --addMateTags --maxSplitCount C --minNonOverlap M --splitterFile FIFO --discordantFile FIFO
  * stdin = name-grouped SAM from `bwa mem`; stdout = the same records with 0x400 on duplicates and MC/MQ appended; the two
  * side files (FIFOs in speedseq, opened up front and streamed) receive the header plus discordant pairs / split reads.
@@ -269,7 +269,7 @@ int main(int argc, char **argv)
 		else if ((!strcmp(argv[i], "-o") || !strcmp(argv[i], "--output")) && i + 1 < argc) { if (!(o.out = fopen(argv[++i], "w"))) return 1; }
 		else { fprintf(stderr, "samblaster: Unrecognized option: %s\n", argv[i]); return 1; }
 	}
-	fprintf(stderr, "samblaster: Version %s (B200 shim over libssq)\n", SB_VERSION);
+	fprintf(stderr, "samblaster: Version %s (GPU shim over libssq)\n", SB_VERSION);
 	if (discfn && !(o.disc = fopen(discfn, "w"))) { fprintf(stderr, "samblaster: Unable to open %s\n", discfn); return 1; }
 	if (splitfn && !(o.split = fopen(splitfn, "w"))) { fprintf(stderr, "samblaster: Unable to open %s\n", splitfn); return 1; }
 	strcpy(cl, "samblaster -i stdin -o stdout");

@@ -5,8 +5,8 @@
 // routines for the host and compare them with the oracle on a box without a GPU (test-only harness,
 // never part of libssq.so: the shipped library has no CPU path).
 //
-// Reference behaviour being reproduced (upstream bwa, not vendored in /root/reference; call site
-// /root/reference/bin/speedseq:438): SURVEY.md §8a rows a4-a7 and Appendix A.
+// Reference behaviour being reproduced (upstream bwa, not vendored in the speedseq tree; call site
+// speedseq/bin/speedseq:438): SURVEY.md §8a rows a4-a7 and Appendix A.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -101,14 +101,15 @@ SSQ_HD void occ4_from_block(const u32 *blk, u64 kk, u64 cnt[4])
 
 // scalar context: one thread does the whole look-up (used by the SA walk, by hostsim, and as the
 // thread-per-read variant of the seeding kernel)
-// one 32-byte rank block (u32 occ[4] + 4 words of 16 symbols) in ONE load instruction: sm_100 has 256-bit global loads, and with
-// every lane on a different line the L1 pipeline charges a wavefront per lane PER INSTRUCTION, so two 128-bit loads cost twice
+// one 32-byte rank block (u32 occ[4] + 4 words of 16 symbols) = one sector, read with two 128-bit loads (the widest global
+// load sm_90 has); both halves are issued before either is used, so a rank query still waits for one memory round trip
 struct Blk32 { u32 c0, c1, c2, c3, w0, w1, w2, w3; };
 SSQ_HD Blk32 load_blk32(const u32 *p)
 {
 	Blk32 b;
 #ifdef __CUDA_ARCH__
-	asm("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+	asm("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+	    "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
 	             : "=r"(b.c0), "=r"(b.c1), "=r"(b.c2), "=r"(b.c3), "=r"(b.w0), "=r"(b.w1), "=r"(b.w2), "=r"(b.w3) : "l"(p));
 #else
 	b.c0 = p[0]; b.c1 = p[1]; b.c2 = p[2]; b.c3 = p[3]; b.w0 = p[4]; b.w1 = p[5]; b.w2 = p[6]; b.w3 = p[7];

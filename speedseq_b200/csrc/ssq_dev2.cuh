@@ -5,7 +5,7 @@
 //   sw_local       local SW in the evaluation order of the 16/8-lane striped kernel (upstream ksw_align2; a11)
 //   mate_rescue    one mem_matesw() call                                                          (a11)
 //   reg2aln        region -> position / CIGAR / NM / MD with the band-doubling loop              (upstream mem_reg2aln; a14)
-// Call site in the reference: inside `$BWA mem`, /root/reference/bin/speedseq:438.  Used by the kernels of
+// Call site in the reference: inside `$BWA mem`, speedseq/bin/speedseq:438.  Used by the kernels of
 // ssq_kernels2.cu (one thread per read / pair / alignment) and, for CPU-side checking only, by tests/hostsim.
 #pragma once
 #include "ssq_dev.cuh"

@@ -9,7 +9,7 @@
 //   sam_line             one SAM record, byte for byte                                   (upstream mem_aln2sam)
 //   sb_*                 samblaster on structured records: signature, discordant and splitter predicates, MC/MQ tags
 //                        (upstream samblaster.cpp markDupsDiscordants / markSplitterUnmappedClipped; SURVEY §8a a16-a19)
-// Reference call sites: `$BWA mem ... | $SAMBLASTER ...` at /root/reference/bin/speedseq:438-439,468-469.
+// Reference call sites: `$BWA mem ... | $SAMBLASTER ...` at speedseq/bin/speedseq:438-439,468-469.
 //
 // Floating point: every double expression below is evaluated as separate IEEE operations (the translation units that include
 // this header are compiled with -fmad=false; the host build has no FMA contraction either), and every transcendental comes from
@@ -454,9 +454,9 @@ SSQ_HD void sam_line(Sink<W> &str, const TextCtx &c, int read, const LS &list, i
 
 // =================================================================================== BAM ====
 // The records of the three streams as BAM (SURVEY.md §8 f1): what `sambamba view -S -f bam` makes of the SAM text, encoded
-// straight from the structured records.  Layout: /root/reference/src/samtools-1.3.1/htslib-1.3.1/sam.c:443-467 (bam_write1 /
+// straight from the structured records.  Layout: speedseq/src/samtools-1.3.1/htslib-1.3.1/sam.c:443-467 (bam_write1 /
 // the in-memory record), bin: htslib/hts.h:580-586 (hts_reg2bin), integer tags take the smallest type that holds the value.
-// Parity is pinned on the reference's OWN tool: tests/golden/ex_bam_*.gz were produced by /root/reference/src/sambamba (v0.5.9)
+// Parity is pinned on the reference's OWN tool: tests/golden/ex_bam_*.gz were produced by speedseq/src/sambamba (v0.5.9)
 // from the oracle's SAM of the example reads (tests/golden/make_bam_golden.py).
 template <bool W> SSQ_HD void bput32(Sink<W> &s, u32 v) { if (W) { s.p[s.n] = (char)v; s.p[s.n + 1] = (char)(v >> 8); s.p[s.n + 2] = (char)(v >> 16); s.p[s.n + 3] = (char)(v >> 24); } s.n += 4; }
 template <bool W> SSQ_HD void bput16(Sink<W> &s, u32 v) { if (W) { s.p[s.n] = (char)v; s.p[s.n + 1] = (char)(v >> 8); } s.n += 2; }

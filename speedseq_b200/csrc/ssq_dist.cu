@@ -2,7 +2,7 @@
 //
 // Alignment shards by whole `bwa mem` batches (the only couplings inside alignment are per-batch: insert-size statistics and
 // read ordinals), the index is replicated: no collective there.  samblaster's rule "the first pair seen with a signature is kept"
-// (`$SAMBLASTER`, /root/reference/bin/speedseq:439) is global over the whole input, though.  With N ranks, batches are dealt
+// (`$SAMBLASTER`, speedseq/bin/speedseq:439) is global over the whole input, though.  With N ranks, batches are dealt
 // round-robin (round k: rank r works on batch k*N + r); in the duplicate stage of a round every rank
 //   1. routes each pair signature (two 64-bit keys) to its OWNER rank = hash(signature) mod N      k_route + stable radix sort by owner
 //   2. all-gathers the N x N count matrix, then exchanges the keys with grouped ncclSend/ncclRecv    16 B per pair out

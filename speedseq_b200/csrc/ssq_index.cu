@@ -1,6 +1,6 @@
 // ssq_index.cu — index loader (PREFIX.{bwt,sa,pac,ann,amb} -> HBM), options, error plumbing.
-// Replaces upstream bwa_idx_load() / mem_opt_init() (start of `$BWA mem`, /root/reference/bin/speedseq:438).
-// On-disk format: the one of the reference's goldens /root/reference/example/data/*.fasta.{amb,ann,pac,bwt,sa}
+// Replaces upstream bwa_idx_load() / mem_opt_init() (start of `$BWA mem`, speedseq/bin/speedseq:438).
+// On-disk format: the one of the reference's goldens speedseq/example/data/*.fasta.{amb,ann,pac,bwt,sa}
 // (SURVEY.md §8c).  Host memory is only a staging area; nothing here computes on the CPU.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -33,9 +33,10 @@ int ssq_use_device(int device)
 	if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) { ssq_set_error("no CUDA device is visible: libssq has no CPU path"); return SSQ_ENOGPU; }
 	if (device < 0 || device >= n) { ssq_set_error("device %d out of range (%d visible)", device, n); return SSQ_ENOGPU; }
 	if (cudaSetDevice(device) != cudaSuccess) { ssq_set_error("cudaSetDevice(%d) failed", device); return SSQ_ENOGPU; }
-	int major = 0;
+	int major = 0, minor = 0;
 	cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
-	if (major != 10) { ssq_set_error("device %d has compute capability %d.x; this library is built for sm_100a only", device, major); return SSQ_ENOGPU; }
+	cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device);
+	if (major != 9 || minor != 0) { ssq_set_error("device %d has compute capability %d.%d; this library is built for sm_90a (H100) only", device, major, minor); return SSQ_ENOGPU; }
 	return SSQ_OK;
 }
 
@@ -174,7 +175,7 @@ extern "C" int ssq_index_load(const char *prefix, int device, ssq_index_t **out)
 		idx->dev.sa = (const u64*)d; idx->dev_bytes += idx->dev.n_sa * 8;
 	}
 	cudaFreeHost(h);
-	{ // denser sample: 180 GB of HBM buys a 4x shorter LF walk per seed occurrence (GRCh37: 6.2 G rows / 8 x 8 B = 6.2 GB)
+	{ // denser sample: a 4x shorter LF walk per seed occurrence for little HBM (GRCh37: 6.2 G rows / 8 x 8 B = 6.2 GB of the H100's 80 GB)
 		const int d = getenv("SSQ_SA_DENSE") ? atoi(getenv("SSQ_SA_DENSE")) : 8;
 		if (d > 0 && d < idx->dev.sa_intv && (d & (d - 1)) == 0) {
 			const u64 nd = idx->dev.seq_len / d + 1;

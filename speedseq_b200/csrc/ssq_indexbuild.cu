@@ -1,12 +1,12 @@
 // ssq_indexbuild.cu — `bwa index` on the GPU: FASTA -> PREFIX.{amb,ann,pac,bwt,sa}.
 //
-// Reference call site: `$BWA index $REF` at /root/reference/bin/speedseq:389 (and :1925); the five files must be
+// Reference call site: `$BWA index $REF` at speedseq/bin/speedseq:389 (and :1925); the five files must be
 // byte-identical to what upstream bwa writes — pinned by the reference's goldens
-// /root/reference/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa} (tests/test_gpu_index.py).
+// speedseq/example/data/human_g1k_v37_20_42220611-42542245.fasta.{amb,ann,pac,bwt,sa} (tests/test_gpu_index.py).
 // Upstream routines replaced (not vendored in the reference tree): bns_fasta2bntseq, bwt_pac2bwt/bwt_bwtgen,
 // bwt_bwtupdate_core, bwt_cal_sa.
 //
-// B200 design: the text T = forward + reverse-complement strand never leaves its 2-bit packing; the suffix array of T$ is
+// Design: the text T = forward + reverse-complement strand never leaves its 2-bit packing; the suffix array of T$ is
 // built by prefix doubling where every round is one LSD radix sort of (rank[i], rank[i+h]) pairs over all suffixes
 // (CUB DeviceRadixSort — HBM-streaming plumbing), ranks are re-derived with a max-scan, and the loop stops when all ranks
 // are distinct (h doubles from 16, so ~log2(longest repeat/16) rounds).  BWT symbols, the occ checkpoints every 128

@@ -1,10 +1,10 @@
-// ssq_kernels.cu — sm_100a kernels of the alignment path and their stream-ordered launch sequence.
+// ssq_kernels.cu — sm_90a kernels of the alignment path and their stream-ordered launch sequence.
 //
-// Stage map (reference: inside `$BWA mem`, /root/reference/bin/speedseq:438; SURVEY.md §8a; measurements in DESIGN.md §5):
+// Stage map (reference: inside `$BWA mem`, speedseq/bin/speedseq:438; SURVEY.md §8a; measurements in DESIGN.md §5):
 //   seeding  a4  default: phase-split kernels — forward walks (k_smem_fwd<1|2>, lane = read), backward sweeps (k_smem_bwd, lane = call),
 //                pass-2 selection (k_smem_p2sel), greedy pass (k_smem_p3), one radix sort on (read, qb, qe) to publish the intervals.
 //                Indexes with >= 2^32 rows: the per-lane state machine k_smem_m<u64> + k_smem_p3 on the 64-byte on-disk rank blocks.
-//                One 256-bit load per rank query of the re-blocked 32-byte sectors.  Bound: random sector reads (L2 / HBM).
+//                Two back-to-back 128-bit loads per rank query of the re-blocked 32-byte sectors.  Bound: random sector reads (L2 / HBM).
 //   k_sa     a5  thread per seed occurrence, LF walk to the load-time densified SA sample.  Same bound.
 //   k_chain / k_chain_coop  a6  per-lane ChainBuilder for reads with <= 16 seeds, warp per read (shared-memory chains, three
 //                capacity levels) above.
@@ -1350,7 +1350,7 @@ struct ssq_batch {
 	u64 call_cap = 0, fl_cap = 0; // split seeding: capacities of the call and forward-list pools
 	cudaEvent_t ev[6], evc[4], evs[2], evx[2], evb[4]; /* evb: around the two backward-sweep launches of the split seeding */ // stage boundaries; chaining tiers; k_smem_m alone; selection kernels of one round // stage boundaries; chaining tiers (light start, heavy start, end)
 	float stage_ms[5];
-	ssq_batch() { memset(&h_cnt, 0, sizeof h_cnt); n_intv = n_seeds = n_tasks = n_regs_total = 0; launches = 0; own_stream = 1; pool_cap = 0; ext_rounds = 0; select_ms = 0.f; { const char *v = getenv("SSQ_SMEM_VARIANT"); smem_variant = v ? atoi(v) : 3; /* phase-split seeding (r02: 48.9 ms vs 59.9 ms for the state machine on the bench workload); indexes without bwt32 use the 64-bit state machine */ } memset(stage_ms, 0, sizeof stage_ms); }
+	ssq_batch() { memset(&h_cnt, 0, sizeof h_cnt); n_intv = n_seeds = n_tasks = n_regs_total = 0; launches = 0; own_stream = 1; pool_cap = 0; ext_rounds = 0; select_ms = 0.f; { const char *v = getenv("SSQ_SMEM_VARIANT"); smem_variant = v ? atoi(v) : 3; /* phase-split seeding (faster than the state machine on the bench workload); indexes without bwt32 use the 64-bit state machine */ } memset(stage_ms, 0, sizeof stage_ms); }
 };
 
 // misc buffer layout (device): [0] pool_n (u64)  [1] work (int) + err (int)  [2..] Counters
@@ -1556,8 +1556,8 @@ static int run_smem(ssq_batch *b)
 	const int warps_per_block = 4, threads = warps_per_block * 32;
 	const size_t smem = variant == 0 ? (size_t)warps_per_block * 2 * (lcap + 1) * sizeof(Intv) : 0;
 	const char *lc_env = getenv("SSQ_LIST_CAP");
-	// shared-memory list entries per lane.  Measured (profiles/r01_smem_sweep.txt): the 32-bit machine is fastest with 6 blocks/SM and
-	// short lists — what the lists do not take stays L1 for the query bytes, the output list and the overflow entries
+	// shared-memory list entries per lane (SSQ_LIST_CAP; SSQ_SMEM_BLOCKS: blocks per SM of the 32-bit machine): short lists leave
+	// what they do not take to L1 for the query bytes, the output list and the overflow entries
 	const bool m32_ = variant == 2 && b->idx->dev.bwt32 != 0 && !getenv("SSQ_SMEM_M64");
 	const int list_cap = variant == 2 && b->idx->dev.seq_len < 0xffffffffull ? (lc_env ? atoi(lc_env) : m32_ ? 6 : 10) : 0;
 	// 32-bit machine (indexes with bwt32): fewer registers, so more blocks per SM when the shared-memory lists leave room for them
@@ -1664,8 +1664,8 @@ static int run_sa(ssq_batch *b)
 	return SSQ_OK;
 }
 
-// The cut between the thread-per-read and the warp-per-read tier of a stage (work items per read), overridable for tests.
-// Measured on B200 (profiles/r01_tier_sweep.txt): the stage time is flat between 32 and 64 and grows on either side.
+// The cut between the thread-per-read and the warp-per-read tier of a stage (work items per read), overridable for tests and
+// sweeps (SSQ_HEAVY_SEEDS, SSQ_HEAVY_TASKS).
 static int tier_threshold(ssq_batch *b, const char *env, int dflt, int *d_thresh)
 {
 	const int v = getenv(env) ? atoi(getenv(env)) : dflt;

@@ -1,5 +1,5 @@
 // ssq_mem.cu — `bwa mem` for one batch through string arrays (upstream mem_process_seqs(); `$BWA mem`,
-// /root/reference/bin/speedseq:438,468): a convenience form of the HBM-resident pipeline in ssq_pipe.cu for callers that hold
+// speedseq/bin/speedseq:438,468): a convenience form of the HBM-resident pipeline in ssq_pipe.cu for callers that hold
 // their reads as separate C strings.  It gathers the strings into the concatenated layout ssq_aligner_run() takes, runs one
 // batch with the samblaster stage switched off, and returns the records as one malloc'd string.  The CLI shim drives a
 // persistent aligner object directly (no per-batch set-up); this entry point creates and frees one per call.
@@ -53,7 +53,7 @@ extern "C" int ssq_mem_batch_sam(const ssq_index_t *idx, const ssq_opts_t *opt, 
 extern "C" void ssq_free(void *p) { free(p); }
 
 // ---- BAM container (host side of f1): BGZF framing and the file header ----
-// BGZF: /root/reference/src/samtools-1.3.1/htslib-1.3.1/bgzf.c:45-63 — a series of gzip members of at most 64 KiB each, every member
+// BGZF: speedseq/src/samtools-1.3.1/htslib-1.3.1/bgzf.c:45-63 — a series of gzip members of at most 64 KiB each, every member
 // carrying its compressed size in a "BC" extra field, and a fixed empty member as end-of-file marker.
 extern "C" int ssq_bgzf_compress(const void *in_, size_t n, int level, int with_eof, void **out, size_t *out_len)
 {

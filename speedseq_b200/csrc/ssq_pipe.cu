@@ -2,12 +2,12 @@
 // resident in HBM.
 //
 // Reference call sites: `$BWA mem -t T [-p] [-C] [-I ..] -R RG REF FQ1 [FQ2] | $SAMBLASTER [--excludeDups] --addMateTags
-// --maxSplitCount C --minNonOverlap M --splitterFile F --discordantFile F` at /root/reference/bin/speedseq:438-439,468-469.
+// --maxSplitCount C --minNonOverlap M --splitterFile F --discordantFile F` at speedseq/bin/speedseq:438-439,468-469.
 // Upstream routines replaced (un-vendored submodules of the reference): mem_process_seqs, mem_pestat, mem_sam_pe, mem_matesw,
 // mem_pair, mem_mark_primary_se, mem_approx_mapq_se, mem_reg2aln, mem_gen_alt, mem_reg2sam, mem_aln2sam; samblaster's
 // markDupsDiscordants, markSplitterUnmappedClipped and its line writer.
 //
-// Stages (all kernels hand-written for sm_100a; CUB only for scans and the radix sort inside the dup-set):
+// Stages (all kernels hand-written for sm_90a; CUB only for scans and the radix sort inside the dup-set):
 //   k_encode        ASCII bases -> one code per base
 //   ssq_batch_run   seeding, SA look-up, chaining, extension                                   (ssq_kernels.cu)
 //   k_dedup         sort / de-duplicate / patch the regions of a read                          (thread per read)
@@ -778,8 +778,8 @@ extern "C" int ssq_sw_local_batch(const ssq_opts_t *opt, int device, uint64_t n,
 
 
 // ============================================================== FASTQ ingest on the device ====
-// Upstream bseq_read() -> kseq_read() (`$BWA mem`, /root/reference/bin/speedseq:438,468); tokenisation rules of the reference's
-// in-tree parser /root/reference/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231, restricted to the layout sequencers
+// Upstream bseq_read() -> kseq_read() (`$BWA mem`, speedseq/bin/speedseq:438,468); tokenisation rules of the reference's
+// in-tree parser speedseq/src/samtools-1.3.1/htslib-1.3.1/htslib/kseq.h:189-231, restricted to the layout sequencers
 // write: four lines per record ('@name[ comment]', bases, '+...', qualities).  Anything else (multi-line records, FASTA, blank
 // lines, unequal files) is REPORTED (SSQ_EFORMAT) and left to the caller's host tokeniser, which handles every legal input.
 //   k_fq_records   thread per record: field extents from the newline positions, checks, name without /1 /2, comment, lengths

@@ -1,6 +1,6 @@
 // ssq_sais.h — suffix array by induced sorting (SA-IS: Nong, Zhang, Chan, "Two efficient algorithms for linear time suffix array
 // construction", 2011), host code.  `ssq_index_build` uses it for references whose 2 x l_pac + 1 suffixes exceed what the GPU
-// prefix-doubling sort of this build holds (2^31 - 2): `$BWA index $REF` on a whole genome, /root/reference/bin/speedseq:386-391
+// prefix-doubling sort of this build holds (2^31 - 2): `$BWA index $REF` on a whole genome, speedseq/bin/speedseq:386-391
 // (SURVEY §8 f3: "GPU suffix sort optional").  Upstream bwa switches to its own incremental BWT construction above 50 Mbp; the
 // index files do not record how the suffix array was obtained.
 //

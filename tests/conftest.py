@@ -10,7 +10,7 @@ import ssq_testlib as T  # noqa: E402
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,10 +1,10 @@
 """Generates tests/golden/ex_bam_{main,spl,disc}.records.gz: the decompressed, coordinate-sorted BAM RECORDS (everything after the
-header and reference table) that the reference's own tool /root/reference/src/sambamba (v0.5.9) produces with the commands of
-/root/reference/bin/speedseq:440-448 —  `sambamba view -S -f bam -l 0 /dev/stdin | sambamba sort` — from the oracle's
+header and reference table) that speedseq's own tool src/sambamba (v0.5.9) produces with the commands of
+speedseq/bin/speedseq:440-448 —  `sambamba view -S -f bam -l 0 /dev/stdin | sambamba sort` — from the oracle's
 `bwa mem -p -R RG | samblaster --excludeDups --addMateTags --maxSplitCount 2 --minNonOverlap 20` over tests/golden/ex_reads_2k.fq.gz
 (the two side streams go through speedseq's gawk step first: SEQ and QUAL become '*', speedseq:443,446; gawk is not installed here, the
 one-line awk program is restated below).  Also writes ex_bam_header.txt: sambamba's rewritten header text.
-Run in the build container (needs /root/reference); the fixtures travel, the reference does not."""
+Needs a speedseq checkout (its path in SPEEDSEQ_CHECKOUT); the tests only read the fixtures."""
 import gzip
 import os
 import struct
@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 import ssq_testlib as T
 
-SB = "/root/reference/src/sambamba"
+SB = os.path.join(os.environ["SPEEDSEQ_CHECKOUT"], "src", "sambamba")
 RG = r"@RG\tID:NA12878\tSM:NA12878\tLB:lib1"
 
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Generates the fixtures under tests/golden/ from the reference checkout.  Run HERE (the container that has
-/root/reference); the GPU box only sees the committed outputs.
+"""Generates the fixtures under tests/golden/ from a speedseq checkout (its path in
+SPEEDSEQ_CHECKOUT); the tests only read the committed outputs.
 
   ex_ref.fa.gz            the reference's example FASTA (example/data/human_g1k_v37_20_42220611-42542245.fasta), gzip'd
   ex_index.sha256.json    sha256 + size of the reference's own golden index files for that FASTA
@@ -13,7 +13,7 @@
 import gzip, hashlib, json, os, subprocess, sys, tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference/example/data"
+REF = os.path.join(os.environ["SPEEDSEQ_CHECKOUT"], "example", "data")
 FA = os.path.join(REF, "human_g1k_v37_20_42220611-42542245.fasta")
 FQ = os.path.join(REF, "NA12878.20slice.30X.fastq.gz")
 

@@ -1,6 +1,6 @@
 """Shared helpers for the test-suite: ctypes bindings of the oracle (oracle/libssqo.so), of the product's C-ABI
 (speedseq_b200/libssq.so) and of the test-only host harness (tests/hostsim/libhostsim.so), plus seeded read/genome
-generators.  Nothing here reads /root/reference at run time."""
+generators.  Nothing here reads a speedseq checkout at run time."""
 import ctypes as C
 import gzip
 import os
@@ -18,6 +18,15 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 from speedseq_b200.capi import SMEM_DT, SEED_DT, SWTASK_DT, SWRES_DT, REG_DT, DUPSIG_DT, SSQ, pack_reads  # noqa: E402,F401  (the product's own bindings)
 ODUPSIG_DT = np.dtype([("pos1", "<u8"), ("pos2", "<u8"), ("strand1", "u1"), ("strand2", "u1"), ("valid", "u1")], align=True)
+
+
+def gpu_visible():
+    """whether libssq sees a CUDA device (device nodes are not a test: a box may expose its GPU under any index); asked in a child
+    process so that loading libssq (and its NCCL) here does not come before torch's own"""
+    if not hasattr(gpu_visible, "n"):
+        r = subprocess.run([sys.executable, "-c", "import ctypes, sys; print(ctypes.CDLL(sys.argv[1]).ssq_device_count())", SSQ_SO], capture_output=True, text=True)
+        gpu_visible.n = int(r.stdout.strip() or 0) if r.returncode == 0 else 0
+    return gpu_visible.n > 0
 
 
 def build_oracle():

@@ -1,7 +1,8 @@
-"""BASELINE config 1 plumbing on the CPU: the reference's UNMODIFIED bin/speedseq with a private config whose $BWA / $SAMBLASTER are the
-oracle CLI (argv-identical to the shims) — once with the reference's sambamba, once with `SAMBAMBA=` the repo's sambamba shim, which
+"""BASELINE config 1 plumbing on the CPU: speedseq's UNMODIFIED bin/speedseq with a private config whose $BWA / $SAMBLASTER are the
+oracle CLI (argv-identical to the shims) — once with speedseq's sambamba, once with `SAMBAMBA=` the repo's sambamba shim, which
 has to hand every call of the script (view / sort of plain SAM and BAM, index) through to the real one.  Same three BAMs both ways.
-Runs only where the reference checkout exists (this build container); the GPU-side runs are profiles/r02_config1_unmodified_speedseq.log."""
+The script, the sambamba binary and the example data are speedseq's own and are not stored here: the test runs where build() staged
+them from a speedseq checkout (see build(), oracle/stage_config1.sh) and skips where none was found."""
 import os
 import subprocess
 
@@ -9,8 +10,8 @@ import pytest
 
 import ssq_testlib as T
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not (os.path.exists(REF + "/bin/speedseq") and os.access(REF + "/src/sambamba", os.X_OK)), reason="no reference checkout on this box")
+REF = os.path.join(T.ROOT, "oracle", "_ref", "stage")
+pytestmark = pytest.mark.skipif(not (os.path.exists(REF + "/bin/speedseq") and os.access(REF + "/src/sambamba", os.X_OK)), reason="build() found no speedseq checkout to stage (set SPEEDSEQ_CHECKOUT)")
 
 
 def test_unmodified_speedseq_runs_with_the_sambamba_shim_in_front_of_the_real_one(tmp_path):

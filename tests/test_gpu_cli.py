@@ -120,7 +120,7 @@ def test_dupset_streaming_equals_one_shot(ssq, oracle):
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# the invocation modes of /root/reference/bin/speedseq that one interleaved single-batch run does not reach: two FASTQ files
+# the invocation modes of speedseq/bin/speedseq that one interleaved single-batch run does not reach: two FASTQ files
 # (:468, the default), -I (:286), -C (:1961), several batches (per-batch insert-size statistics + global read ordinals), smart
 # pairing with unpaired reads, gz input, and the fused samblaster stage behind the same two executables
 def _records(b):

@@ -1,7 +1,7 @@
 """`ssq_index_build` beyond the device sort's 2^31 - 2 suffixes builds the suffix array on the host (induced sorting, 64-bit indices,
 csrc/ssq_sais.h) and writes the same five files; no GPU is touched.  SSQ_INDEX_HOST forces that path for any size (1: narrowest entry
 type, 40: the 5-byte entries a whole genome gets, 64: 8-byte entries), so it is pinned here, on the CPU, on the reference's own golden index
-(/root/reference/example/data/*.fasta.{amb,ann,pac,bwt,sa}) and against the oracle's builder on synthetic multi-contig genomes."""
+(speedseq/example/data/*.fasta.{amb,ann,pac,bwt,sa}) and against the oracle's builder on synthetic multi-contig genomes."""
 import ctypes as C
 import gzip
 import hashlib
@@ -56,7 +56,7 @@ def test_host_index_equals_oracle_on_synthetic_genomes(ssq_lib_cpu, oracle, tmp_
 
 def test_small_reference_still_needs_the_gpu(ssq_lib_cpu, tmp_path, monkeypatch):
     """without the knob a reference the device sort holds goes to the device: on a box without a GPU that is an error, not a silent CPU build"""
-    if os.path.exists("/dev/nvidia0"):
+    if T.gpu_visible():
         pytest.skip("a GPU is present")
     monkeypatch.delenv("SSQ_INDEX_HOST", raising=False)
     fa = str(tmp_path / "ex.fa")

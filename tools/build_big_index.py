@@ -22,7 +22,7 @@ import bench
 
 glen = int(sys.argv[1]) if len(sys.argv) > 1 else 2_200_000_000
 n_pairs = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
-cache = os.path.join(ROOT, "data_cache")
+cache = bench.cache_dir()
 lib = C.CDLL(os.path.join(ROOT, "speedseq_b200", "libssq.so"))
 lib.ssq_index_build.argtypes = [C.c_char_p, C.c_char_p, C.c_int]
 lib.ssq_last_error.restype = C.c_char_p

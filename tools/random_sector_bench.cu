@@ -1,8 +1,9 @@
 // How fast can this device serve dependent random 32-byte sector reads — the access pattern of FM-index seeding (every backward
 // extension reads the rank blocks its previous result names)?  Each thread walks M independent chains of random 32-B reads over a
 // table of the given size; the sweep over resident warps and chains per thread gives the ceiling `k_smem_bwd` is to be held against
-// (bench.py's `roofline.peak` stays the streaming copy bandwidth of MEASURED_PEAKS.json, as the contract asks).
-// build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/random_sector_bench tools/random_sector_bench.cu
+// (bench.py's `roofline.peak` stays the data-sheet HBM bandwidth).  Each 32-B sector is read with two 128-bit loads, as
+// load_blk32() in ssq_dev.cuh does on sm_90.
+// build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/random_sector_bench tools/random_sector_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -12,7 +13,7 @@
 __device__ __forceinline__ uint32_t ld32B(const void *p)
 {
 	uint32_t a, b, c, d, e, f, g, h;
-	asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d), "=r"(e), "=r"(f), "=r"(g), "=r"(h) : "l"(p));
+	asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\tld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d), "=r"(e), "=r"(f), "=r"(g), "=r"(h) : "l"(p));
 	return a ^ b ^ c ^ d ^ e ^ f ^ g ^ h;
 }
 __device__ __forceinline__ uint64_t mix(uint64_t x) { x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; return x ^ (x >> 33); }

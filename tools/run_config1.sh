@@ -2,12 +2,12 @@
 # BASELINE config 1: the reference's own example (`example/run_speedseq.sh` step 1) through the UNMODIFIED bin/speedseq with a
 # private config.  usage: tools/run_config1.sh <oracle|b200|b200_fused|b200_bam> <reference-checkout> <workdir>
 #   oracle     : $BWA/$SAMBLASTER = oracle/ssqo (CPU)
-#   b200       : $BWA/$SAMBLASTER = speedseq_b200/bin/{bwa,samblaster} (needs a B200; the reference checkout may be the staged one
-#                of tools/stage_config1.sh)
+#   b200       : $BWA/$SAMBLASTER = speedseq_b200/bin/{bwa,samblaster} (needs an H100; the reference checkout may be the staged one
+#                of oracle/stage_config1.sh)
 #   b200_fused : + the config stanza of INTEGRATION.md §2: samblaster's stage runs on the device inside `bwa mem`
 #   b200_bam   : + SSQ_FUSE_BAM and $SAMBAMBA = speedseq_b200/bin/sambamba: the main records never exist as text
 set -e
-MODE=${1:-oracle}; REF=${2:-/root/reference}; W=${3:-/tmp/ssq_config1}
+MODE=${1:-oracle}; REF=${2:?usage: tools/run_config1.sh MODE SPEEDSEQ_CHECKOUT [WORKDIR]}; W=${3:-/tmp/ssq_config1}
 ROOT=$(cd "$(dirname "$0")/.." && pwd)
 mkdir -p "$W/bin"; cd "$W"
 if [ "${MODE#b200}" != "$MODE" ]; then BWA=$ROOT/speedseq_b200/bin/bwa; SB=$ROOT/speedseq_b200/bin/samblaster

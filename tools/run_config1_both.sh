@@ -1,5 +1,5 @@
 #!/bin/bash
-# BASELINE config 1 four ways through the UNMODIFIED bin/speedseq: oracle CLI (CPU), the B200 shims, the B200 shims with the fused
+# BASELINE config 1 four ways through the UNMODIFIED bin/speedseq: oracle CLI (CPU), the GPU shims, the GPU shims with the fused
 # samblaster stage, and those with the main records as BAM runs into the `sambamba` shim; then the three BAMs of each GPU run against
 # the oracle run's: records (sambamba view) and header minus the @PG
 # lines (they carry executable paths) must be identical.  usage: tools/run_config1_both.sh [staged-reference] [workdir]

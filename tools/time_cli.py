@@ -17,7 +17,7 @@ from speedseq_b200 import capi
 
 n_reads = int(sys.argv[1]) if len(sys.argv) > 1 else 4_000_000
 glen = int(sys.argv[2]) if len(sys.argv) > 2 else 63025520
-cache = os.path.join(ROOT, "data_cache")
+cache = bench.cache_dir()
 s = capi.SSQ()
 fa, g = bench.ensure_reference(cache, glen, lambda f: s.index_build(f, None, 0))
 fq = os.path.join(cache, "cli_%d.fq" % n_reads)

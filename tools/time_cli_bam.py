@@ -21,8 +21,8 @@ from speedseq_b200 import capi
 n_reads = int(sys.argv[1]) if len(sys.argv) > 1 else 2_000_000
 glen = int(sys.argv[2]) if len(sys.argv) > 2 else 63025520
 REAL = sys.argv[3] if len(sys.argv) > 3 else os.path.join(ROOT, "oracle", "_ref", "stage", "src", "sambamba")
-assert os.access(REAL, os.X_OK), "the reference's sambamba is needed (tools/stage_config1.sh stages it)"
-cache = os.path.join(ROOT, "data_cache")
+assert os.access(REAL, os.X_OK), "the reference's sambamba is needed (oracle/stage_config1.sh stages it)"
+cache = bench.cache_dir()
 s = capi.SSQ()
 fa, g = bench.ensure_reference(cache, glen, lambda f: s.index_build(f, None, 0))
 fq = os.path.join(cache, "cli_%d.fq" % n_reads)

@@ -8,7 +8,7 @@ import ssq_testlib as T
 import bench
 
 n_pairs = int(sys.argv[1]) if len(sys.argv) > 1 else 200000
-cache = os.path.join(ROOT, "data_cache")
+cache = bench.cache_dir()
 s = T.SSQ(); o = T.Oracle()
 s.opts[29] = bench.usable_cores()  # host threads (opt.n_threads)
 fa, g = bench.ensure_reference(cache, bench.GENOME_LEN, lambda f: s.index_build(f))
