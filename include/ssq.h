@@ -270,6 +270,20 @@ int ssq_bam_header(const ssq_index_t *idx, const char *sam_header_text, int sort
  * tag order inside @SQ / @RG / @PG lines); free with ssq_free */
 int ssq_bam_header_text(const char *sam_header_text, int sorted, char **out);
 int ssq_bgzf_compress(const void *in, size_t n, int level, int with_eof, void **out, size_t *out_len);           /* free with ssq_free */
+/* The same BGZF file layout, compressed on the device (csrc/ssq_bgzf.cu): the input is cut into 0xff00-byte payloads from its start
+ * exactly as ssq_bgzf_compress cuts it, each payload becomes one gzip member (BC extra field, CRC-32, ISIZE) holding one deflate block
+ * (stored, fixed or dynamic Huffman, whichever is smallest), so the decompressed file and its block boundaries are the host path's;
+ * only the deflate bytes differ.  Level 0 writes stored blocks; levels 1-9 (and -1) all run the one device encoder.  The output is a
+ * function of the input bytes and of level == 0 alone — not of how the input is split across calls, the launch or the stream.
+ * An object owns device buffers, a stream and pinned staging, reused across calls; one host thread at a time. */
+typedef struct ssq_bgzf ssq_bgzf_t;
+int ssq_bgzf_create(int device, ssq_bgzf_t **out);
+/* host buffers: same contract, block cutting and EOF handling as ssq_bgzf_compress; *out malloc'd, free with ssq_free */
+int ssq_bgzf_deflate(ssq_bgzf_t *z, const void *in, size_t n, int level, int with_eof, void **out, size_t *out_len);
+/* device buffers, on the object's stream (returns after it is done); SSQ_ECAP + *needed when out_cap is too small */
+int ssq_bgzf_deflate_dev(ssq_bgzf_t *z, const void *d_in, size_t n, int level, int with_eof, void *d_out, size_t out_cap, size_t *out_len, size_t *needed);
+void *ssq_bgzf_stream(ssq_bgzf_t *z);               /* cudaStream_t of the object, for event timing */
+void ssq_bgzf_free(ssq_bgzf_t *z);
 /* the sorted runs of consecutive batches -> one sorted record stream (stable: equal keys keep batch order); free with ssq_free */
 int ssq_bam_merge_runs(int n_runs, const void *const *runs, const size_t *lens, void **out, size_t *out_len);
 

@@ -207,3 +207,37 @@ class SSQ:
     def aligner_free(self, al):
         self.lib.ssq_aligner_free(al)
 
+    # ---- BGZF compression on the device (ssq_bgzf_*) ----
+    def bgzf_create(self, device=0):
+        L = self.lib
+        L.ssq_bgzf_stream.restype = C.c_void_p
+        L.ssq_bgzf_stream.argtypes = [C.c_void_p]
+        L.ssq_bgzf_free.argtypes = [C.c_void_p]
+        L.ssq_free.argtypes = [C.c_void_p]
+        h = C.c_void_p()
+        self.ck(L.ssq_bgzf_create(C.c_int(device), C.byref(h)), "ssq_bgzf_create")
+        return h
+
+    def bgzf_deflate(self, z, data, level=6, with_eof=1):
+        """bytes (or a buffer) in host memory -> the BGZF file as bytes"""
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        out, n = C.c_void_p(), C.c_size_t(0)
+        self.ck(self.lib.ssq_bgzf_deflate(z, _ptr(buf), C.c_size_t(len(data)), C.c_int(level), C.c_int(with_eof), C.byref(out), C.byref(n)), "ssq_bgzf_deflate")
+        r = C.string_at(out, n.value)
+        self.lib.ssq_free(out)
+        return r
+
+    def bgzf_deflate_dev(self, z, d_in, n, d_out, out_cap, level=6, with_eof=1):
+        """device pointers (ints) -> (rc, out_len, needed); rc is SSQ_ECAP (-5) when out_cap is too small"""
+        ln, need = C.c_size_t(0), C.c_size_t(0)
+        rc = self.lib.ssq_bgzf_deflate_dev(z, C.c_void_p(d_in), C.c_size_t(n), C.c_int(level), C.c_int(with_eof), C.c_void_p(d_out), C.c_size_t(out_cap), C.byref(ln), C.byref(need))
+        if rc not in (0, -5):
+            self.ck(rc, "ssq_bgzf_deflate_dev")
+        return rc, int(ln.value), int(need.value)
+
+    def bgzf_stream(self, z):
+        return self.lib.ssq_bgzf_stream(z)
+
+    def bgzf_free(self, z):
+        self.lib.ssq_bgzf_free(z)
+

@@ -156,9 +156,14 @@ static void merge_sources(src_t *s, int n_src, sink_fn sink, void *ctx)
 	free(h);
 }
 
-/* ---- BGZF output on several threads ---- */
-typedef struct { FILE *fp; const uint8_t *buf; size_t n; int threads, level; } flush_t;
-typedef struct { FILE *fp; uint8_t *buf, *alt; size_t n, cap; int threads, level; pthread_t bg; int bg_live; flush_t job; } bgzf_out_t;
+/* ---- BGZF output on several threads, or on the device (SSQ_BGZF_GPU=1) ---- */
+typedef struct { FILE *fp; const uint8_t *buf; size_t n; int threads, level; ssq_bgzf_t *z; } flush_t;
+typedef struct { FILE *fp; uint8_t *buf, *alt; size_t n, cap; int threads, level; ssq_bgzf_t *z; pthread_t bg; int bg_live; flush_t job; } bgzf_out_t;
+static void write_member_bytes(FILE *fp, void *p, size_t n)
+{
+	if (fwrite(p, 1, n, fp) != n) { perror("sambamba (GPU shim): write"); exit(1); }
+	ssq_free(p);
+}
 typedef struct { const uint8_t *in; size_t n; int level; void *out; size_t out_len; int rc; } job_t;
 static void *job_main(void *a) { job_t *j = (job_t*)a; j->rc = ssq_bgzf_compress(j->in, j->n, j->level, 0, &j->out, &j->out_len); return 0; }
 static void *flush_main(void *a) /* one buffer: compressed in slices on `threads` threads, written in order */
@@ -169,6 +174,12 @@ static void *flush_main(void *a) /* one buffer: compressed in slices on `threads
 	int nj = f->threads, k;
 	const size_t blk = 0xff00; /* the payload of one block: slices end on block boundaries, so the file is the same for any thread count */
 	size_t per, at = 0;
+	if (f->z) { /* the whole buffer in one call on the device */
+		void *out = 0; size_t len = 0;
+		if (ssq_bgzf_deflate(f->z, f->buf, f->n, f->level, 0, &out, &len)) { fprintf(stderr, "sambamba (GPU shim): BGZF compression on the device (SSQ_BGZF_GPU=1) failed: %s\n", ssq_last_error()); exit(1); }
+		write_member_bytes(f->fp, out, len);
+		return 0;
+	}
 	per = ((f->n / blk + (size_t)nj) / (size_t)nj) * blk;
 	for (k = 0; k < nj && at < f->n; ++k) { jobs[k].in = f->buf + at; jobs[k].n = f->n - at < per ? f->n - at : per; jobs[k].level = f->level; jobs[k].out = 0; jobs[k].out_len = 0; at += jobs[k].n; }
 	nj = k;
@@ -177,8 +188,7 @@ static void *flush_main(void *a) /* one buffer: compressed in slices on `threads
 	for (k = 1; k < nj; ++k) pthread_join(th[k], 0);
 	for (k = 0; k < nj; ++k) {
 		if (jobs[k].rc) { fprintf(stderr, "sambamba (GPU shim): BGZF compression failed: %s\n", ssq_last_error()); exit(1); }
-		if (fwrite(jobs[k].out, 1, jobs[k].out_len, f->fp) != jobs[k].out_len) { perror("sambamba (GPU shim): write"); exit(1); }
-		ssq_free(jobs[k].out);
+		write_member_bytes(f->fp, jobs[k].out, jobs[k].out_len);
 	}
 	return 0;
 }
@@ -190,7 +200,7 @@ static void bgzf_flush(bgzf_out_t *o)
 	uint8_t *t;
 	if (!o->n) return;
 	bgzf_wait(o);
-	o->job.fp = o->fp; o->job.buf = o->buf; o->job.n = o->n; o->job.threads = o->threads; o->job.level = o->level;
+	o->job.fp = o->fp; o->job.buf = o->buf; o->job.n = o->n; o->job.threads = o->threads; o->job.level = o->level; o->job.z = o->z;
 	if (pthread_create(&o->bg, 0, flush_main, &o->job)) flush_main(&o->job); else o->bg_live = 1;
 	t = o->buf; o->buf = o->alt; o->alt = t;
 	o->n = 0;
@@ -222,6 +232,14 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 	char *hdr_text, *hdr_sorted = 0;
 	bgzf_out_t o;
 	char **spill_fn = 0;
+	ssq_bgzf_t *z = 0;
+	{ /* SSQ_BGZF_GPU=1: the sorted file is compressed on SSQ_DEVICE (an explicit choice: its deflate bytes differ from zlib's) */
+		const char *g = getenv("SSQ_BGZF_GPU");
+		if (g && !strcmp(g, "1")) {
+			const char *dv = getenv("SSQ_DEVICE");
+			if (ssq_bgzf_create(dv && dv[0] ? atoi(dv) : 0, &z)) { fprintf(stderr, "sambamba (GPU shim): SSQ_BGZF_GPU=1 asks for BGZF compression on the GPU, but: %s\n", ssq_last_error()); return 1; }
+		}
+	}
 	/* header text without the markers of the private stream */
 	hdr_text = (char*)malloc(body + 1);
 	{ size_t w = 0, p = 0; while (p < body) { const char *nl = (const char*)memchr(h->p + p, '\n', body - p); const size_t l = (size_t)(nl + 1 - (h->p + p)); if (strncmp(h->p + p, "@CO\tssq-", 8) != 0) { memcpy(hdr_text + w, h->p + p, l); w += l; } p += l; } hdr_text[w] = 0; }
@@ -262,8 +280,11 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 	for (i = 0; i < n_mem; ++i) spill[n_spill + i] = mem[i];
 	/* output: header block(s), records, end-of-file block */
 	memset(&o, 0, sizeof o);
+	o.z = z;
 	if (!(o.fp = fopen(out_fn, "wb"))) { fprintf(stderr, "sambamba (GPU shim): cannot create %s: %s\n", out_fn, strerror(errno)); return 1; }
-	o.threads = threads < 1 ? 1 : threads > 64 ? 64 : threads; o.level = level; o.cap = (size_t)0xff00 * 256 * (size_t)o.threads; o.buf = (uint8_t*)malloc(o.cap); o.alt = (uint8_t*)malloc(o.cap);
+	o.threads = threads < 1 ? 1 : threads > 64 ? 64 : threads; o.level = level;
+	if (z) { o.cap = (size_t)0xff00 * 1024; o.buf = (uint8_t*)ssq_host_alloc(o.cap); o.alt = (uint8_t*)ssq_host_alloc(o.cap); } /* pinned: full-rate copies to the device */
+	else { o.cap = (size_t)0xff00 * 256 * (size_t)o.threads; o.buf = (uint8_t*)malloc(o.cap); o.alt = (uint8_t*)malloc(o.cap); }
 	if (!o.buf || !o.alt) { fprintf(stderr, "sambamba (GPU shim): out of memory\n"); return 1; }
 	if (ssq_bam_header_text(hdr_text, 1, &hdr_sorted)) { fprintf(stderr, "sambamba (GPU shim): %s\n", ssq_last_error()); return 1; }
 	{ /* "BAM\1", text, reference table from the @SQ lines */
@@ -290,6 +311,7 @@ static int sort_runs(head_t *h, size_t body, const char *out_fn, int threads, in
 	{ void *eofb = 0; size_t el = 0; if (ssq_bgzf_compress("", 0, level, 1, &eofb, &el)) { fprintf(stderr, "sambamba (GPU shim): %s\n", ssq_last_error()); return 1; } fwrite(eofb, 1, el, o.fp); ssq_free(eofb); }
 	if (fclose(o.fp)) { perror("sambamba (GPU shim): close"); return 1; }
 	for (i = 0; i < n_spill; ++i) { fclose(spill[i].fp); unlink(spill_fn[i]); }
+	if (z) { ssq_host_free(o.buf); ssq_host_free(o.alt); ssq_bgzf_free(z); }
 	return 0;
 }
 

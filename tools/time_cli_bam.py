@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""The align step's whole chain to a sorted BAM file, wall clock, two ways (speedseq:438-441):
+"""The align step's whole chain to a sorted BAM file, wall clock, three ways (speedseq:438-441):
   text : bwa mem | samblaster | sambamba view -S -f bam -l 0 | sambamba sort      — shims for the first two, the REFERENCE'S sambamba
   bam  : the same command line with SSQ_FUSE_BAM and the `sambamba` shim          — the main records never exist as text
-and a check that both files hold the same records in the same order (`sambamba view` of both, by the reference's sambamba), i.e. the
+  bamz : bam + SSQ_BGZF_GPU=1: the shim compresses the sorted file on the GPU     — `bwa` and `sambamba` share the GPU by time slicing
+and a check that all files hold the same records in the same order (`sambamba view` of both, by the reference's sambamba), i.e. the
 device-side encode + sort + the shim's merge against the reference's own tool on a few million reads.
 usage: time_cli_bam.py [n_reads] [genome_bp] [path of the real sambamba]"""
 import hashlib
@@ -49,9 +50,10 @@ for tag, env, with_sb in (("bwa mem (fused, text) > /dev/null", {}, 0), ("bwa me
         assert p1.wait(timeout=300) == 0
     print("%-46s %6.2f s" % (tag, time.time() - t0), flush=True)
 res = {}
-for tag, env, sambamba in (("text + reference sambamba", {}, REAL), ("BAM runs + sambamba shim", {"SSQ_FUSE_BAM": "1"}, os.path.join(B, "sambamba"))):
+for tag, env, sambamba in (("text + reference sambamba", {}, REAL), ("BAM runs + sambamba shim", {"SSQ_FUSE_BAM": "1"}, os.path.join(B, "sambamba")),
+                           ("BAM runs + shim, BGZF on the GPU", {"SSQ_FUSE_BAM": "1", "SSQ_BGZF_GPU": "1"}, os.path.join(B, "sambamba"))):
     e = dict(os.environ, SSQ_FUSE_SAMBLASTER=" ".join(sb_args), SSQ_SAMBAMBA_REAL=REAL, **env)
-    out = os.path.join(cache, "cli_%s.bam" % ("text" if not env else "runs"))
+    out = os.path.join(cache, "cli_%s.bam" % ("text" if not env else "runs" if len(env) == 1 else "runs_gpuz"))
     tmp = os.path.join(cache, "sort_tmp"); os.makedirs(tmp, exist_ok=True)
     t0 = time.time()
     p1 = subprocess.Popen([os.path.join(B, "bwa"), "mem", "-t", "8", "-p", "-R", RG, fa, fq], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, env=e)
@@ -70,7 +72,7 @@ for tag, env, sambamba in (("text + reference sambamba", {}, REAL), ("BAM runs +
     assert v.wait() == 0
     hdr = subprocess.run([REAL, "view", "-H", out], stdout=subprocess.PIPE, check=True).stdout
     res[tag] = (h.hexdigest(), n_rec, b"".join(l for l in hdr.splitlines(True) if not l.startswith(b"@PG")))
-    print("%-28s %6.2f s  %6.2f M reads/s to a sorted BAM of %d MB, %d records  (check: %.1f s)" % (tag, dt, n_reads / dt / 1e6, os.path.getsize(out) >> 20, n_rec, time.time() - t1), flush=True)
-a, b = res.values()
-assert a == b, "the two BAM files differ: %r %r" % (a[:2], b[:2])
-print("records (sambamba view of both files) and header minus @PG identical: md5 %s, %d records" % (a[0], a[1]))
+    print("%-32s %6.2f s  %6.2f M reads/s to a sorted BAM of %d bytes, %d records  (check: %.1f s)" % (tag, dt, n_reads / dt / 1e6, os.path.getsize(out), n_rec, time.time() - t1), flush=True)
+a, b, c = res.values()
+assert a == b == c, "the BAM files differ: %r %r %r" % (a[:2], b[:2], c[:2])
+print("records (sambamba view of all three files) and header minus @PG identical: md5 %s, %d records" % (a[0], a[1]))
