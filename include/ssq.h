@@ -105,6 +105,17 @@ typedef struct { int32_t score, te, qe, score2, te2, tb, qb; } ssq_swl_result_t;
 int ssq_sw_local_batch(const ssq_opts_t *opt, int device, uint64_t n, const ssq_swl_task_t *tasks, const uint8_t *qbuf, uint64_t qbuf_len,
                        const uint8_t *tbuf, uint64_t tbuf_len, ssq_swl_result_t *out);
 
+/* Banded global alignment with traceback.  Replaces upstream ksw_global2() as called from bwa_gen_cigar2() (CIGAR generation inside
+ * `$BWA mem`, speedseq:438); the same warp routine as the pipeline's CIGAR stage (csrc/ssq_warp.cuh: sw_global_warp), one warp per
+ * problem.  Task i aligns qbuf[q_off, +qlen) against tbuf[t_off, +tlen) in a band of half-width w; its CIGAR (op | len << 4, ops
+ * 0 M, 1 I, 2 D) goes to cig[cig_off, +cig_cap).  cig_cap == 0: score only (n_cigar = 0).  n_cigar = -1: the CIGAR needs more than
+ * cig_cap operations (nothing is cut short).  Every task must satisfy 1 <= qlen <= SSQ_MAX_READ_LEN, 1 <= tlen <= 2048, w >= 0 and
+ * |tlen - qlen| <= w (the end cell lies in the band), and its buffers must be in range; otherwise SSQ_EINVAL and nothing runs. */
+typedef struct { uint64_t q_off, t_off; int32_t qlen, tlen, w, cig_cap; uint64_t cig_off; } ssq_swg_task_t;
+typedef struct { int32_t score, n_cigar; } ssq_swg_result_t;
+int ssq_sw_global_batch(const ssq_opts_t *opt, int device, uint64_t n, const ssq_swg_task_t *tasks, const uint8_t *qbuf, uint64_t qbuf_len,
+                        const uint8_t *tbuf, uint64_t tbuf_len, uint32_t *cig, uint64_t cig_len, ssq_swg_result_t *out);
+
 /* Chains after seeding + SA lookup + chaining + chain filter.  Replaces upstream mem_chain() +
  * mem_chain_flt() (speedseq:438).  Flattened: read i owns chains [read_chain_off[i], read_chain_off[i+1]),
  * chain c owns seeds [chain_seed_off[c], chain_seed_off[c+1]). */

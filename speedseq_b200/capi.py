@@ -16,8 +16,13 @@ SWRES_DT = np.dtype([("score", "<i4"), ("qle", "<i4"), ("tle", "<i4"), ("gtle", 
 REG_DT = np.dtype([("rb", "<i8"), ("re", "<i8"), ("qb", "<i4"), ("qe", "<i4"), ("rid", "<i4"), ("score", "<i4"), ("truesc", "<i4"),
                    ("w", "<i4"), ("seedcov", "<i4"), ("seedlen0", "<i4"), ("frac_rep", "<f4"), ("read_id", "<i4")])
 DUPSIG_DT = np.dtype([("pos1", "<u8"), ("pos2", "<u8"), ("strand1", "u1"), ("strand2", "u1"), ("valid", "u1"), ("pad", "u1", (5,))])
+SWLTASK_DT = np.dtype([("q_off", "<u8"), ("t_off", "<u8"), ("qlen", "<i4"), ("tlen", "<i4"), ("xtra", "<i4"), ("pad", "<i4")])
+SWLRES_DT = np.dtype([("score", "<i4"), ("te", "<i4"), ("qe", "<i4"), ("score2", "<i4"), ("te2", "<i4"), ("tb", "<i4"), ("qb", "<i4")])
+SWGTASK_DT = np.dtype([("q_off", "<u8"), ("t_off", "<u8"), ("qlen", "<i4"), ("tlen", "<i4"), ("w", "<i4"), ("cig_cap", "<i4"), ("cig_off", "<u8")])
+SWGRES_DT = np.dtype([("score", "<i4"), ("n_cigar", "<i4")])
 
 assert SMEM_DT.itemsize == 32 and SEED_DT.itemsize == 16 and SWTASK_DT.itemsize == 40 and REG_DT.itemsize == 56 and DUPSIG_DT.itemsize == 24
+assert SWLTASK_DT.itemsize == 32 and SWLRES_DT.itemsize == 28 and SWGTASK_DT.itemsize == 40 and SWGRES_DT.itemsize == 8
 
 
 def _ptr(a):
@@ -128,10 +133,32 @@ class SSQ:
         self.ck(self.lib.ssq_sa_lookup_batch(idx, C.c_uint64(len(rows)), _ptr(rows), _ptr(pos)), "ssq_sa_lookup_batch")
         return pos
 
-    def sw_extend_batch(self, tasks, qbuf, tbuf, device=0):
+    def make_opts(self, **kw):
+        """ssq_opts_t: the defaults with the named scoring fields (a, b, o_del, e_del, o_ins, e_ins) replaced"""
+        o = (C.c_int32 * self.OPTS_WORDS)()
+        C.memmove(o, self.opts, C.sizeof(o))
+        for k, v in kw.items():
+            o[("a", "b", "o_del", "e_del", "o_ins", "e_ins").index(k)] = int(v)
+        return o
+
+    def sw_extend_batch(self, tasks, qbuf, tbuf, device=0, opts=None):
         res = np.zeros(len(tasks), SWRES_DT)
-        self.ck(self.lib.ssq_sw_extend_batch(self.opts, C.c_int(device), C.c_uint64(len(tasks)), _ptr(tasks), _ptr(qbuf), C.c_uint64(len(qbuf)), _ptr(tbuf),
+        self.ck(self.lib.ssq_sw_extend_batch(opts or self.opts, C.c_int(device), C.c_uint64(len(tasks)), _ptr(tasks), _ptr(qbuf), C.c_uint64(len(qbuf)), _ptr(tbuf),
                                              C.c_uint64(len(tbuf)), _ptr(res)), "ssq_sw_extend_batch")
+        return res
+
+    def sw_local_batch(self, tasks, qbuf, tbuf, device=0, opts=None):
+        """ksw_align2 problems (SWLTASK_DT) -> SWLRES_DT"""
+        res = np.zeros(len(tasks), SWLRES_DT)
+        self.ck(self.lib.ssq_sw_local_batch(opts or self.opts, C.c_int(device), C.c_uint64(len(tasks)), _ptr(tasks), _ptr(qbuf), C.c_uint64(len(qbuf)), _ptr(tbuf),
+                                            C.c_uint64(len(tbuf)), _ptr(res)), "ssq_sw_local_batch")
+        return res
+
+    def sw_global_batch(self, tasks, qbuf, tbuf, cig, device=0, opts=None):
+        """ksw_global2 problems (SWGTASK_DT) -> SWGRES_DT; the CIGAR of task i is written to cig[cig_off, +n_cigar) (a uint32 array)"""
+        res = np.zeros(len(tasks), SWGRES_DT)
+        self.ck(self.lib.ssq_sw_global_batch(opts or self.opts, C.c_int(device), C.c_uint64(len(tasks)), _ptr(tasks), _ptr(qbuf), C.c_uint64(len(qbuf)), _ptr(tbuf),
+                                             C.c_uint64(len(tbuf)), _ptr(cig), C.c_uint64(len(cig)), _ptr(res)), "ssq_sw_global_batch")
         return res
 
     def chain_batch(self, idx, seq, off):

@@ -30,7 +30,8 @@ SSQ_HD int score_of(const ssq_opts_t &o, int a, int b) { return (a > 3 || b > 3)
 #define SSQ_MINUS_INF (-0x40000000)
 struct GlobalScratch { i32 *h, *e; uint8_t *z; long zcap; }; // h/e: qlen+1 each; z: n_col*tlen (may be null when no CIGAR is wanted)
 
-// query q[0..qlen), target t[0..tlen) (arrays of codes). cigar (op | len<<4) written reversed-then-fixed into cig[0..*n_cig)
+// query q[0..qlen), target t[0..tlen) (arrays of codes). cigar (op | len<<4) written reversed-then-fixed into cig[0..*n_cig);
+// *n_cig = -1 when the operations do not fit in cig_cap (reported, never cut short)
 SSQ_HD int sw_global(const ssq_opts_t &o, int qlen, const uint8_t *q, int tlen, const uint8_t *t, int w, const GlobalScratch &S, u32 *cig, int cig_cap, int *n_cig)
 {
 	const int o_del = o.o_del, e_del = o.e_del, o_ins = o.o_ins, e_ins = o.e_ins, oe_del = o_del + e_del, oe_ins = o_ins + e_ins;
@@ -72,8 +73,9 @@ SSQ_HD int sw_global(const ssq_opts_t &o, int qlen, const uint8_t *q, int tlen, 
 	const int score = S.h[qlen];
 	if (S.z && cig && n_cig) { // traceback, operations collected from the end then reversed
 		int n = 0, which = 0;
+		bool full = false;
 		i = tlen - 1; k = (i + w + 1 < qlen ? i + w + 1 : qlen) - 1;
-#define PUSH_OP(op_, len_) do { if (n == 0 || (int)(cig[n - 1] & 0xf) != (op_)) { if (n < cig_cap) cig[n++] = (u32)(len_) << 4 | (op_); } else cig[n - 1] += (u32)(len_) << 4; } while (0)
+#define PUSH_OP(op_, len_) do { if (n == 0 || (int)(cig[n - 1] & 0xf) != (op_)) { if (n < cig_cap) cig[n++] = (u32)(len_) << 4 | (op_); else full = true; } else cig[n - 1] += (u32)(len_) << 4; } while (0)
 		while (i >= 0 && k >= 0) {
 			which = S.z[(size_t)i * n_col + (k - (i > w ? i - w : 0))] >> (which << 1) & 3;
 			if (which == 0) { PUSH_OP(0, 1); --i; --k; }
@@ -84,7 +86,7 @@ SSQ_HD int sw_global(const ssq_opts_t &o, int qlen, const uint8_t *q, int tlen, 
 		if (k >= 0) PUSH_OP(1, k + 1);
 #undef PUSH_OP
 		for (i = 0; i < n >> 1; ++i) { u32 x = cig[i]; cig[i] = cig[n - 1 - i]; cig[n - 1 - i] = x; }
-		*n_cig = n;
+		*n_cig = full ? -1 : n;
 	}
 	return score;
 }
@@ -138,6 +140,7 @@ SSQ_HD bool gen_cigar(const DevIndex &ix, const ssq_opts_t &o, int w_, int l_que
 		if (!cig) g.z = 0;
 		else if ((long)(l_query < 2 * w + 1 ? l_query : 2 * w + 1) * rlen > g.zcap) { if (n_cig) *n_cig = -1; return false; } // traceback matrix would not fit: reported, never silent
 		*score = sw_global(o, l_query, S.qbuf, rlen, S.rbuf, w, g, cig, cig_cap, n_cig);
+		if (cig && n_cig && *n_cig < 0) return false; // more operations than cig_cap: reported like the matrix overflow above
 	}
 	if (NM && cig && n_cig) {
 		int k, x, y, u, n_mm = 0, n_gap = 0;

@@ -244,6 +244,32 @@ __global__ void __launch_bounds__(128) k_sw_local_tasks(ssq_opts_t opt, u64 n, c
 	if (lane == 0) { ssq_swl_result_t o; o.score = r.score; o.te = r.te; o.qe = r.qe; o.score2 = r.score2; o.te2 = r.te2; o.tb = r.tb; o.qb = r.qb; out[t] = o; }
 }
 
+// kernel-level entry: ksw_global2 problems (banded global DP + traceback) over caller-supplied sequences, shaped like k_cigar_warp:
+// persistent warps take tasks from a counter, each owns a traceback slab of zcap bytes (parity target: the oracle's ssqo_ksw_global2)
+__global__ void __launch_bounds__(128) k_sw_global_tasks(ssq_opts_t opt, u64 n, const ssq_swg_task_t *__restrict__ tk, const uint8_t *__restrict__ qbuf,
+                                                         const uint8_t *__restrict__ tbuf, u32 *cig, ssq_swg_result_t *out, uint8_t *zslabs, long zcap, unsigned long long *work)
+{
+	__shared__ WarpGlSmem sm[4];
+	const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+	WarpGlSmem &W = sm[wid];
+	uint8_t *z = zslabs + ((size_t)blockIdx.x * 4 + wid) * (size_t)zcap;
+	for (;;) {
+		unsigned long long t = 0;
+		if (lane == 0) t = atomicAdd(work, 1ull);
+		t = __shfl_sync(WFULL, t, 0);
+		if (t >= n) break;
+		const ssq_swg_task_t k = tk[t];
+		__syncwarp();
+		for (int i = lane; i < k.qlen; i += 32) W.q[i] = qbuf[k.q_off + i];
+		for (int i = lane; i < k.tlen; i += 32) W.r[i] = tbuf[k.t_off + i];
+		__syncwarp();
+		const int w = k.w < k.qlen + k.tlen ? k.w : k.qlen + k.tlen; // (a band wider than both sequences changes nothing; keeps i + w + 1 in range)
+		int n_cig = 0;
+		const int score = sw_global_warp(opt, k.qlen, k.tlen, w, W, z, zcap, k.cig_cap ? cig + k.cig_off : 0, k.cig_cap, &n_cig, lane);
+		if (lane == 0) { ssq_swg_result_t o; o.score = score; o.n_cigar = n_cig; out[t] = o; }
+	}
+}
+
 __global__ void __launch_bounds__(128) k_sb(PipeView V)
 {
 	const int u = blockIdx.x * blockDim.x + threadIdx.x;
@@ -341,12 +367,22 @@ extern "C" void ssq_aligner_free(ssq_aligner_t *a)
 	delete a;
 }
 
+// SSQ_RESCUE_SPLIT=0 selects the 16-lane form of the byte-mode local SW (ssq_warp.cuh); written on every call that runs it, so that
+// a value does not outlive the environment it was read from (unset: 1, the 32-lane form)
+static int set_rescue_split()
+{
+	const char *s = getenv("SSQ_RESCUE_SPLIT");
+	const int v = s ? atoi(s) : 1;
+	CK(cudaMemcpyToSymbol(ssq_rescue_split, &v, sizeof v));
+	return SSQ_OK;
+}
+
 extern "C" int ssq_aligner_create(const ssq_index_t *idx, const ssq_opts_t *opt, const ssq_sb_opts_t *sb, const char *rg_id, ssq_aligner_t **out)
 {
 	if (!idx || !opt || !out) return SSQ_EINVAL;
 	int rc = ssq_use_device(idx->device);
 	if (rc) return rc;
-	if (getenv("SSQ_RESCUE_SPLIT")) { const int v = atoi(getenv("SSQ_RESCUE_SPLIT")); CK(cudaMemcpyToSymbol(ssq_rescue_split, &v, sizeof v)); } // 0: the 16-lane form of the local SW (ssq_warp.cuh)
+	if ((rc = set_rescue_split())) return rc;
 	ssq_aligner *a = new ssq_aligner();
 	a->idx = idx; a->opt = *opt; a->device = idx->device; a->b = 0; a->comm = 0; a->dups = 0; a->own_dups = 1; a->turn = -1; a->want_bam = 0; a->bam_blank_side = 1; a->bam_len[0] = a->bam_len[1] = a->bam_len[2] = 0; a->n_lines_total = 0; a->computed = 0; a->n_reads = 0;
 	a->rescue_spec = !(getenv("SSQ_RESCUE_SPEC") && !atoi(getenv("SSQ_RESCUE_SPEC"))); // 0: every rescue alignment computed inside the sequential replay
@@ -760,6 +796,7 @@ extern "C" int ssq_sw_local_batch(const ssq_opts_t *opt, int device, uint64_t n,
 	int rc = ssq_use_device(device);
 	if (rc) return rc;
 	if (n == 0) return SSQ_OK;
+	if ((rc = set_rescue_split())) return rc;
 	int b_cap = 1;
 	for (u64 i = 0; i < n; ++i) {
 		if (tasks[i].qlen < 0 || tasks[i].qlen > SSQ_MAX_READ_LEN || tasks[i].tlen < 0 || tasks[i].q_off + tasks[i].qlen > qbuf_len || tasks[i].t_off + tasks[i].tlen > tbuf_len) { ssq_set_error("ssq_sw_local_batch: task %llu out of range", (unsigned long long)i); return SSQ_EINVAL; }
@@ -773,6 +810,46 @@ extern "C" int ssq_sw_local_batch(const ssq_opts_t *opt, int device, uint64_t n,
 	k_sw_local_tasks<<<(unsigned)((n + 3) / 4), 128>>>(*opt, n, dt.as<ssq_swl_task_t>(), dq.as<uint8_t>(), dtb.as<uint8_t>(), dout.as<ssq_swl_result_t>(), dbl.as<u64>(), b_cap);
 	CK(cudaGetLastError());
 	CK(cudaMemcpy(out, dout.p, n * sizeof(ssq_swl_result_t), cudaMemcpyDeviceToHost));
+	return SSQ_OK;
+}
+
+extern "C" int ssq_sw_global_batch(const ssq_opts_t *opt, int device, uint64_t n, const ssq_swg_task_t *tasks, const uint8_t *qbuf, uint64_t qbuf_len,
+                                   const uint8_t *tbuf, uint64_t tbuf_len, uint32_t *cig, uint64_t cig_len, ssq_swg_result_t *out)
+{
+	if (!opt || (n && (!tasks || !qbuf || !tbuf || !out))) return SSQ_EINVAL;
+	long zcap = 1;
+	for (u64 i = 0; i < n; ++i) { // every task is checked before anything runs: outside these bounds the traceback would leave the band
+		const ssq_swg_task_t &k = tasks[i];
+		const int dl = k.tlen > k.qlen ? k.tlen - k.qlen : k.qlen - k.tlen;
+		if (k.qlen < 1 || k.qlen > SSQ_MAX_READ_LEN || k.tlen < 1 || k.tlen > WG_RCAP || k.w < 0 || dl > k.w || k.cig_cap < 0 || k.q_off + k.qlen > qbuf_len ||
+		    k.t_off + k.tlen > tbuf_len || (k.cig_cap && (!cig || k.cig_off + k.cig_cap > cig_len))) {
+			ssq_set_error("ssq_sw_global_batch: task %llu out of range", (unsigned long long)i); return SSQ_EINVAL;
+		}
+		const long zn = (long)(k.qlen < 2 * (long)k.w + 1 ? k.qlen : 2 * (long)k.w + 1) * k.tlen;
+		if (k.cig_cap && zn > zcap) zcap = zn;
+	}
+	int rc = ssq_use_device(device);
+	if (rc) return rc;
+	if (n == 0) return SSQ_OK;
+	int dev = 0, n_sm = 0;
+	CK(cudaGetDevice(&dev));
+	CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+	const u64 want = (n + 3) / 4, blocks = want < (u64)n_sm * 6 ? want : (u64)n_sm * 6; // 4 warps per block, at most 24 warps per SM
+	u64 cig_words = 0;
+	for (u64 i = 0; i < n; ++i) if (tasks[i].cig_cap && tasks[i].cig_off + tasks[i].cig_cap > cig_words) cig_words = tasks[i].cig_off + tasks[i].cig_cap;
+	DBuf dt, dq, dtb, dcig, dout, dz, dwork;
+	if (dt.need(n * sizeof(ssq_swg_task_t)) || dq.need(qbuf_len + 16) || dtb.need(tbuf_len + 16) || dcig.need(cig_words * 4 + 16) || dout.need(n * sizeof(ssq_swg_result_t)) ||
+	    dz.need(blocks * 4 * (size_t)zcap) || dwork.need(8)) return SSQ_ENOMEM;
+	CK(cudaMemcpy(dt.p, tasks, n * sizeof(ssq_swg_task_t), cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(dq.p, qbuf, qbuf_len, cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(dtb.p, tbuf, tbuf_len, cudaMemcpyHostToDevice));
+	CK(cudaMemset(dwork.p, 0, 8));
+	k_sw_global_tasks<<<(unsigned)blocks, 128>>>(*opt, n, dt.as<ssq_swg_task_t>(), dq.as<uint8_t>(), dtb.as<uint8_t>(), dcig.as<u32>(), dout.as<ssq_swg_result_t>(), dz.as<uint8_t>(), zcap,
+	                                             dwork.as<unsigned long long>());
+	CK(cudaGetLastError());
+	CK(cudaMemcpy(out, dout.p, n * sizeof(ssq_swg_result_t), cudaMemcpyDeviceToHost));
+	for (u64 i = 0; i < n; ++i) // only the CIGARs that came back whole
+		if (out[i].n_cigar > 0) CK(cudaMemcpy(cig + tasks[i].cig_off, dcig.as<u32>() + tasks[i].cig_off, (size_t)out[i].n_cigar * 4, cudaMemcpyDeviceToHost));
 	return SSQ_OK;
 }
 

@@ -15,8 +15,10 @@
 //                    band, rows sequential, F by a 5-step shuffle scan; the traceback byte of every cell is the same function of
 //                    the same integers as in the scalar loop, rows of it are written coalesced.
 // Both keep everything hot in shared memory (DP rows, query profile / sequences); only the traceback matrix and the list of
-// sub-optimal rows live in per-warp global scratch.  Results are bit-identical to the scalar routines (tests: test_gpu_pipe.py,
-// test_gpu_parity.py::test_sw_local / test_cigar against the oracle).
+// sub-optimal rows live in per-warp global scratch.  Results are bit-identical to the scalar routines (tests against the oracle:
+// test_gpu_sw_kernels.py through the kernel-level entries ssq_sw_global_batch / ssq_sw_local_batch, test_gpu_parity.py::
+// test_sw_local_striped_order, and whole records in test_gpu_pipe.py; test_sw_kernels_cpu.py checks the scalar routines on the
+// same problems).
 #pragma once
 #include "ssq_dev3.cuh"
 
@@ -547,7 +549,8 @@ __device__ LocalRes rescue_task_warp(const PipeView &V, const RTask &t, int p, W
 struct WarpGlSmem { i32 H[2][QMAX_W + 16], E[QMAX_W + 16]; uint8_t q[QMAX_W], r[WG_RCAP]; };
 
 // banded global alignment of W.q[0..qlen) vs W.r[0..tlen), traceback into cig (lane 0 writes).  z: per-warp global scratch of
-// zcap bytes (null / too small: score only when cig == null, else *n_cig = -1).  Same contract and results as sw_global()
+// zcap bytes (null / too small: score only when cig == null, else *n_cig = -1); *n_cig = -1 as well when the operations do not fit
+// in cig_cap.  Same contract and results as sw_global()
 __device__ int sw_global_warp(const ssq_opts_t &o, int qlen, int tlen, int w, WarpGlSmem &W, uint8_t *z, long zcap, u32 *cig, int cig_cap, int *n_cig, int lane, unsigned long long *cells = 0)
 {
 	const int o_del = o.o_del, e_del = o.e_del, o_ins = o.o_ins, e_ins = o.e_ins, oe_del = o_del + e_del, oe_ins = o_ins + e_ins;
@@ -613,7 +616,8 @@ __device__ int sw_global_warp(const ssq_opts_t &o, int qlen, int tlen, int w, Wa
 		int n = 0;
 		if (lane == 0) {
 			int which = 0, i = tlen - 1, k = (i + w + 1 < qlen ? i + w + 1 : qlen) - 1;
-#define PUSH_OP(op_, len_) do { if (n == 0 || (int)(cig[n - 1] & 0xf) != (op_)) { if (n < cig_cap) cig[n++] = (u32)(len_) << 4 | (op_); } else cig[n - 1] += (u32)(len_) << 4; } while (0)
+			bool full = false;
+#define PUSH_OP(op_, len_) do { if (n == 0 || (int)(cig[n - 1] & 0xf) != (op_)) { if (n < cig_cap) cig[n++] = (u32)(len_) << 4 | (op_); else full = true; } else cig[n - 1] += (u32)(len_) << 4; } while (0)
 			while (i >= 0 && k >= 0) {
 				which = z[(size_t)i * n_col + (k - (i > w ? i - w : 0))] >> (which << 1) & 3;
 				if (which == 0) { PUSH_OP(0, 1); --i; --k; }
@@ -624,6 +628,7 @@ __device__ int sw_global_warp(const ssq_opts_t &o, int qlen, int tlen, int w, Wa
 			if (k >= 0) PUSH_OP(1, k + 1);
 #undef PUSH_OP
 			for (i = 0; i < n >> 1; ++i) { const u32 x = cig[i]; cig[i] = cig[n - 1 - i]; cig[n - 1 - i] = x; }
+			if (full) n = -1; // more operations than cig_cap: reported, never cut short (gen_cigar_warp returns false)
 		}
 		n = __shfl_sync(WFULL, n, 0);
 		*n_cig = n;
