@@ -33,6 +33,7 @@ extern "C" {
 #define SSQ_ECUDA    (-6)  /* a CUDA call failed; see ssq_last_error() */
 #define SSQ_ELEN     (-7)  /* a read is longer than SSQ_MAX_READ_LEN */
 #define SSQ_EFORMAT  (-8)  /* FASTQ text the device tokeniser does not take (see ssq_aligner_upload_fastq); use the host tokeniser */
+#define SSQ_EDATA    (-9)  /* compressed input is corrupt or truncated; see ssq_last_error() */
 
 #define SSQ_MAX_READ_LEN 255
 
@@ -295,6 +296,28 @@ int ssq_bgzf_deflate(ssq_bgzf_t *z, const void *in, size_t n, int level, int wit
 int ssq_bgzf_deflate_dev(ssq_bgzf_t *z, const void *d_in, size_t n, int level, int with_eof, void *d_out, size_t out_cap, size_t *out_len, size_t *needed);
 void *ssq_bgzf_stream(ssq_bgzf_t *z);               /* cudaStream_t of the object, for event timing */
 void ssq_bgzf_free(ssq_bgzf_t *z);
+/* gzip decoding on the device (csrc/ssq_gunzip.cu): one deflate stream is split into chunks of chunk_bytes compressed bytes and
+ * decoded chunk-parallel (speculative decoding from searched block starts, checked link by link and repaired, then verified with
+ * CRC-32 and ISIZE).  End of stream as zlib's gzread: concatenated members are one stream, bytes after a member that do not start
+ * with 1f 8b are ignored, an empty input is an empty output.  Corrupt or truncated input is SSQ_EDATA, with the compressed offset in
+ * ssq_last_error(); never a short output.  An object holds about 1.6 GB of device memory (1 GB of chunk slots, 512 MB of window
+ * text, the window's input), a stream and pinned staging; one host thread at a time.  Without a usable GPU create returns
+ * SSQ_ENOGPU. */
+typedef struct ssq_gunzip ssq_gunzip_t;
+int ssq_gunzip_create(int device, size_t chunk_bytes, ssq_gunzip_t **out); /* chunk_bytes 0 = default (32 KB); 256 B .. 4 MB */
+/* streaming: in[0, n) continues the object's stream (final: nothing follows it).  Decodes whole windows into out, keeps text it
+ * could not deliver for the next call (which then consumes nothing), *used = leading input bytes the caller drops before the next
+ * call, which passes the rest followed by more input; *done once the stream has ended and all its text was delivered.  After *done
+ * or an error the next call starts a new stream.  Unless
+ * final, nothing is decoded (and *used = 0) before n reaches one window of input (GZ_MAXCH chunks + 1 MB, 33 MB by default). */
+int ssq_gunzip_inflate(ssq_gunzip_t *g, const void *in, size_t n, int final, size_t *used, void *out, size_t out_cap, size_t *out_len, int *done);
+/* a whole stream, device buffers, on the object's stream (returns after it is done); SSQ_ECAP with *out_len = the text's size
+ * when it does not fit.  Independent of the streaming state. */
+int ssq_gunzip_inflate_dev(ssq_gunzip_t *g, const void *d_in, size_t n, void *d_out, size_t out_cap, size_t *out_len);
+/* since create: chunks decoded, chunks started at a searched sync point, chunks decoded again after a broken link, windows */
+int ssq_gunzip_stats(const ssq_gunzip_t *g, int64_t out[4]);
+void *ssq_gunzip_stream(ssq_gunzip_t *g);           /* cudaStream_t of the object, for event timing */
+void ssq_gunzip_free(ssq_gunzip_t *g);
 /* the sorted runs of consecutive batches -> one sorted record stream (stable: equal keys keep batch order); free with ssq_free */
 int ssq_bam_merge_runs(int n_runs, const void *const *runs, const size_t *lens, void **out, size_t *out_len);
 

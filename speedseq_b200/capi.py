@@ -268,3 +268,59 @@ class SSQ:
     def bgzf_free(self, z):
         self.lib.ssq_bgzf_free(z)
 
+    # ---- gzip decoding on the device (ssq_gunzip_*) ----
+    def gunzip_create(self, device=0, chunk_bytes=0):
+        L = self.lib
+        L.ssq_gunzip_stream.restype = C.c_void_p
+        L.ssq_gunzip_stream.argtypes = [C.c_void_p]
+        L.ssq_gunzip_free.argtypes = [C.c_void_p]
+        L.ssq_gunzip_stats.argtypes = [C.c_void_p, C.c_void_p]
+        L.ssq_gunzip_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        L.ssq_gunzip_inflate_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+        h = C.c_void_p()
+        self.ck(L.ssq_gunzip_create(C.c_int(device), C.c_size_t(chunk_bytes), C.byref(h)), "ssq_gunzip_create")
+        return h
+
+    def gunzip_inflate(self, g, data, final, out):
+        """one streaming call into the uint8 array `out`: -> (rc, used, text bytes, done); rc is 0 or SSQ_EDATA (-9)"""
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        used, ln, done = C.c_size_t(0), C.c_size_t(0), C.c_int(0)
+        rc = self.lib.ssq_gunzip_inflate(g, _ptr(buf), C.c_size_t(len(data)), C.c_int(final), C.byref(used), _ptr(out), C.c_size_t(len(out)), C.byref(ln), C.byref(done))
+        if rc not in (0, -9):
+            self.ck(rc, "ssq_gunzip_inflate")
+        return rc, int(used.value), out[:ln.value].tobytes(), bool(done.value)
+
+    def gunzip(self, g, data, piece=1 << 62, out_cap=64 << 20):
+        """a whole stream through the streaming call, `piece` more bytes per call after the unconsumed rest: -> (rc, text)"""
+        pend, at, text, out = bytearray(), 0, [], np.empty(max(out_cap, 1), np.uint8)
+        while True:
+            if at < len(data):
+                pend += data[at:at + piece]
+                at += piece
+            rc, used, t, done = self.gunzip_inflate(g, pend, int(at >= len(data)), out[:out_cap])
+            if rc:
+                return rc, b"".join(text)
+            text.append(t)
+            del pend[:used]
+            if done:
+                return 0, b"".join(text)
+
+    def gunzip_inflate_dev(self, g, d_in, n, d_out, out_cap):
+        """device pointers (ints) -> (rc, out_len); rc is 0, SSQ_ECAP (-5) or SSQ_EDATA (-9)"""
+        ln = C.c_size_t(0)
+        rc = self.lib.ssq_gunzip_inflate_dev(g, C.c_void_p(d_in), C.c_size_t(n), C.c_void_p(d_out), C.c_size_t(out_cap), C.byref(ln))
+        if rc not in (0, -5, -9):
+            self.ck(rc, "ssq_gunzip_inflate_dev")
+        return rc, int(ln.value)
+
+    def gunzip_stats(self, g):
+        """(chunks decoded, chunks started at a searched sync point, chunks decoded again after a broken link, windows) since create"""
+        s = (C.c_int64 * 4)()
+        self.ck(self.lib.ssq_gunzip_stats(g, s), "ssq_gunzip_stats")
+        return tuple(s)
+
+    def gunzip_stream(self, g):
+        return self.lib.ssq_gunzip_stream(g)
+
+    def gunzip_free(self, g):
+        self.lib.ssq_gunzip_free(g)

@@ -22,31 +22,86 @@
 #include <string.h>
 #include <pthread.h>
 #include <unistd.h>
-#include <zlib.h>
+#include <errno.h>
+#include <fcntl.h>
 #include "ssq.h"
 #include "ssq_fuse.h"
 
 #define SHIM_VERSION "0.7.12-r1039" /* the bwa release whose behaviour libssq reproduces (DESIGN.md §3) */
 
 /* ---------------------------------------------------------------- FASTQ/FASTA reader ---- */
-typedef struct { gzFile fp; unsigned char *buf; int beg, end, eof, last; } fq_t;
+/* one input file (or stdin): gzip (first bytes 1f 8b) is inflated on the device by its own ssq_gunzip object, anything else is
+ * read as it is.  Corrupt or truncated gzip ends the program with the file's name, never a short input. */
+typedef struct { const char *fn; int fd, gz, eof, done; ssq_gunzip_t *g; unsigned char *z; size_t zlen, zcap; } in_t;
+static void in_more(in_t *r) /* read until the compressed buffer is full (grown first if it is) or the input ends */
+{
+	if (r->zlen == r->zcap) {
+		r->zcap = r->zcap ? r->zcap * 2 : 1u << 20;
+		if (!(r->z = (unsigned char*)realloc(r->z, r->zcap))) { fprintf(stderr, "[E::bwa] out of memory reading `%s'\n", r->fn); exit(1); }
+	}
+	while (!r->eof && r->zlen < r->zcap) {
+		const ssize_t n = read(r->fd, r->z + r->zlen, r->zcap - r->zlen);
+		if (n < 0 && errno == EINTR) continue;
+		if (n < 0) { fprintf(stderr, "[E::bwa] cannot read `%s': %s\n", r->fn, strerror(errno)); exit(1); }
+		if (n == 0) r->eof = 1; else r->zlen += (size_t)n;
+	}
+}
+static int in_open(in_t *r, const char *fn, int device)
+{
+	int rc;
+	memset(r, 0, sizeof *r);
+	r->fn = fn;
+	if ((r->fd = strcmp(fn, "-") ? open(fn, O_RDONLY) : 0) < 0) return -1;
+	in_more(r);
+	if (r->zlen >= 2 && r->z[0] == 0x1f && r->z[1] == 0x8b) {
+		if ((rc = ssq_gunzip_create(device, 0, &r->g))) { fprintf(stderr, "[E::bwa] `%s' is gzipped and the device gzip decoder is not available (%d): %s\n", fn, rc, ssq_last_error()); exit(1); }
+		r->gz = 1;
+	}
+	return 0;
+}
+/* up to cap bytes of text into buf; 0 at the end of the input */
+static size_t in_read(in_t *r, void *buf, size_t cap)
+{
+	if (!r->gz) {
+		if (r->zlen) {
+			const size_t k = r->zlen < cap ? r->zlen : cap;
+			memcpy(buf, r->z, k); memmove(r->z, r->z + k, r->zlen - k); r->zlen -= k;
+			return k;
+		}
+		for (;;) {
+			const ssize_t n = r->eof ? 0 : read(r->fd, buf, cap);
+			if (n < 0 && errno == EINTR) continue;
+			if (n < 0) { fprintf(stderr, "[E::bwa] cannot read `%s': %s\n", r->fn, strerror(errno)); exit(1); }
+			if (n == 0) r->eof = 1;
+			return (size_t)n;
+		}
+	}
+	while (!r->done) {
+		size_t used = 0, len = 0;
+		const int rc = ssq_gunzip_inflate(r->g, r->z, r->zlen, r->eof, &used, buf, cap, &len, &r->done);
+		if (rc) { fprintf(stderr, "[E::bwa] `%s': %s\n", r->fn, ssq_last_error()); exit(1); }
+		memmove(r->z, r->z + used, r->zlen - used); r->zlen -= used;
+		if (len) return len;
+		if (!used && !r->eof) in_more(r); /* the decoder wants a whole window of input */
+	}
+	return 0;
+}
+
+typedef struct { in_t *in; unsigned char *buf; int beg, end, eof, last; } fq_t;
 typedef struct { char *s; size_t l, m; } str_t;
 typedef struct { str_t name, comment, seq, qual; } rec_t;
 
-/* raw text of an input for the device tokeniser (ssq_aligner_upload_fastq): page-locked, refilled from the (possibly gzipped) file */
-typedef struct { gzFile fp; char *buf; size_t len, cap; int eof; } raw_t;
-static int raw_open(raw_t *r, const char *fn)
+/* raw text of an input for the device tokeniser (ssq_aligner_upload_fastq): page-locked, refilled from the input */
+typedef struct { in_t in; char *buf; size_t len, cap; int eof; } raw_t;
+static int raw_open(raw_t *r, const char *fn, int device)
 {
 	memset(r, 0, sizeof *r);
-	r->fp = strcmp(fn, "-") ? gzopen(fn, "r") : gzdopen(0, "r");
-	if (!r->fp) return -1;
-	gzbuffer(r->fp, 1 << 20);
-	return 0;
+	return in_open(&r->in, fn, device);
 }
 static void raw_fill(raw_t *r, size_t want)
 {
 	while (!r->eof && r->len < want) {
-		int n;
+		size_t n;
 		if (r->cap < want) {
 			const size_t ncap = want + want / 4;
 			char *nb = (char*)ssq_host_alloc(ncap);
@@ -54,18 +109,18 @@ static void raw_fill(raw_t *r, size_t want)
 			if (r->len) memcpy(nb, r->buf, r->len);
 			ssq_host_free(r->buf); r->buf = nb; r->cap = ncap;
 		}
-		n = gzread(r->fp, r->buf + r->len, (unsigned)((r->cap - r->len) < (1u << 30) ? (r->cap - r->len) : (1u << 30)));
-		if (n <= 0) r->eof = 1; else r->len += (size_t)n;
+		n = in_read(&r->in, r->buf + r->len, r->cap - r->len);
+		if (n == 0) r->eof = 1; else r->len += n;
 	}
 }
-/* hand the rest of a raw reader (its unconsumed bytes, then the file) to the host tokeniser */
+/* hand the rest of a raw reader (its unconsumed bytes, then the input) to the host tokeniser */
 static fq_t *fq_from_raw(raw_t *r)
 {
 	fq_t *f = (fq_t*)calloc(1, sizeof(fq_t));
 	const size_t cap = r->len > (1u << 18) ? r->len : (1u << 18);
-	f->fp = r->fp; f->buf = (unsigned char*)malloc(cap);
+	f->in = &r->in; f->buf = (unsigned char*)malloc(cap);
 	if (r->len) memcpy(f->buf, r->buf, r->len);
-	f->beg = 0; f->end = (int)r->len; f->eof = 0; /* a further gzread reports the end again */
+	f->beg = 0; f->end = (int)r->len; f->eof = 0; /* a further read reports the end again */
 	ssq_host_free(r->buf); r->buf = 0; r->len = r->cap = 0;
 	return f;
 }
@@ -73,7 +128,7 @@ static inline int fq_getc(fq_t *f)
 {
 	if (f->beg >= f->end) {
 		if (f->eof) return -1;
-		f->beg = 0; f->end = gzread(f->fp, f->buf, 1 << 18);
+		f->beg = 0; f->end = (int)in_read(f->in, f->buf, 1 << 18);
 		if (f->end <= 0) { f->eof = 1; f->end = 0; return -1; }
 	}
 	return f->buf[f->beg++];
@@ -360,10 +415,10 @@ static int main_mem(int argc, char **argv, const char *prog)
 	if ((rc = ssq_index_load(argv[optind], device, &idx))) die("ssq_index_load", rc);
 	if ((rc = ssq_aligner_create(idx, &opt, fused ? &sb : 0, rg_id, &al))) die("ssq_aligner_create", rc);
 	if (g_bam && (rc = ssq_aligner_set_bam(al, 1, 1))) die("ssq_aligner_set_bam", rc);
-	if (raw_open(&R1, argv[optind + 1])) { fprintf(stderr, "[E::main_mem] fail to open file `%s'.\n", argv[optind + 1]); return 1; }
+	if (raw_open(&R1, argv[optind + 1], device)) { fprintf(stderr, "[E::main_mem] fail to open file `%s'.\n", argv[optind + 1]); return 1; }
 	if (optind + 2 < argc) {
 		if (smart_pe) fprintf(stderr, "[W::main_mem] when '-p' is in use, the second query file is ignored.\n");
-		else { if (raw_open(&R2, argv[optind + 2])) { fprintf(stderr, "[E::main_mem] fail to open file `%s'.\n", argv[optind + 2]); return 1; } paired = 1; two_files = 1; }
+		else { if (raw_open(&R2, argv[optind + 2], device)) { fprintf(stderr, "[E::main_mem] fail to open file `%s'.\n", argv[optind + 2]); return 1; } paired = 1; two_files = 1; }
 	}
 	dev_ingest = !(getenv("SSQ_HOST_FASTQ") && atoi(getenv("SSQ_HOST_FASTQ"))); /* the device tokenises; the host tokeniser takes over when the text is not four-line FASTQ */
 	if (!dev_ingest) { f1 = fq_from_raw(&R1); if (two_files) f2 = fq_from_raw(&R2); }
