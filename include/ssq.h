@@ -62,12 +62,36 @@ void ssq_opts_default(ssq_opts_t *o);
  * and uploads them to `device`. */
 typedef struct ssq_index ssq_index_t;
 /* `$BWA index $REF` (speedseq/bin/speedseq:389): FASTA (plain or gz) -> PREFIX.{amb,ann,pac,bwt,sa}, byte-identical
- * to the reference's goldens for example/data; suffix sorting, BWT, occ checkpoints and SA sampling run on `device`.
- * References beyond the device sort's 2^31 - 2 suffixes (1.07 Gbp; a whole human genome has 6.2 G) are indexed on the host
- * instead — induced sorting with 5-byte entries, same files, no GPU touched (about 15 bytes of host memory per base pair:
- * 45 GB and 51 min for a 3.1 Gbp reference on 8 cores).
- * prefix == NULL means prefix = fasta.  Replaces upstream bwa_idx_build(). */
-int ssq_index_build(const char *fasta, const char *prefix, int device);
+ * to the reference's goldens for example/data and independent of the path that built them.  prefix == NULL means
+ * prefix = fasta.  Replaces upstream bwa_idx_build().  Two ways to sort the suffixes of forward + reverse-complement text:
+ *   2 device sort (csrc/ssq_sapass.cuh): 5 bytes of device memory per suffix for the rank array plus a working budget, fewer
+ *     than 2^40 suffixes; the first sort runs in passes over buckets of leading 12-mers, then doubling rounds over the
+ *     suffixes still tied.  GRCh37 (3.1 Gbp): 31 GB of rank array.
+ *   3 host: induced sorting with 5-byte entries, no GPU touched (about 15 bytes of host memory per base pair).
+ *     SSQ_INDEX_HOST=1 (or 40 / 64: entry width) forces it under the automatic choice.
+ * The automatic choice (path 0) reads the device's *free* memory and leaves 1 GB + 1/32 of it to other users: path 2 when
+ * the rank array, the text and a working budget of at least max(256 MB, 1.25 B per suffix: at most 32 first-sort passes) fit;
+ * else path 3 (also for a reference past 2^31 - 2 suffixes with no usable device; a smaller one with no device gives
+ * SSQ_ENOGPU).  Each first-sort pass reads the whole text, so a budget near that floor costs more passes.  A bucket of
+ * suffixes sharing their first 12 bases that exceeds the budget is sorted on its own; when even that does not fit in free
+ * device memory the call returns SSQ_ENOMEM rather than falling back.  Measured costs: DESIGN.md §8. */
+int ssq_index_build(const char *fasta, const char *prefix, int device); /* = ssq_index_build_ex(fasta, prefix, device, NULL, NULL) */
+typedef struct {
+	int32_t path;        /* 0 auto, 2 device sort, 3 host (1 is not a path: SSQ_EINVAL) */
+	int32_t pad;
+	uint64_t work_bytes; /* path 2: working budget beyond rank array, text and bucket counts; 0 = from free memory at the start */
+} ssq_index_build_opts_t;
+typedef struct {
+	int32_t path, pad;   /* the path that ran */
+	int64_t passes, rounds, chunks; /* path 2: first-sort passes, doubling rounds, chunks over all rounds */
+	int64_t unresolved_first, largest_group; /* suffixes still tied after the first sort, largest such group */
+	int64_t oversize_groups;  /* buckets / groups larger than the budget, each sorted on its own */
+	int64_t peak_device_bytes; /* path 2: most device memory held at once (rank array, text and working set) */
+	int64_t ranges;      /* path 2: finalisation ranges (BWT / checkpoints / SA samples written per range of rows) */
+} ssq_index_build_stats_t;
+/* opt / st may be NULL.  SSQ_EINVAL: a path the reference is too large for; SSQ_ENOMEM (path 2): device memory short, the
+ * message gives the sizes.  When path 0 took the host path, ssq_last_error() says why (empty when it was forced). */
+int ssq_index_build_ex(const char *fasta, const char *prefix, int device, const ssq_index_build_opts_t *opt, ssq_index_build_stats_t *st);
 int ssq_index_load(const char *prefix, int device, ssq_index_t **out);
 void ssq_index_free(ssq_index_t *idx);
 /* what: 0 l_pac, 1 seq_len(=2*l_pac), 2 primary, 3 n_seqs, 4 bwt words, 5 n_sa, 6 device bytes, 7 bytes per rank query (32|64),

@@ -75,6 +75,15 @@ def pack_reads(names, seqs, quals=None, comments=None, paired=1, n_processed=0):
     return r, keep
 
 
+class IndexBuildOpts(C.Structure):
+    _fields_ = [("path", C.c_int32), ("pad", C.c_int32), ("work_bytes", C.c_uint64)]
+
+
+class IndexBuildStats(C.Structure):
+    _fields_ = [("path", C.c_int32), ("pad", C.c_int32)] + [(k, C.c_int64) for k in
+                ("passes", "rounds", "chunks", "unresolved_first", "largest_group", "oversize_groups", "peak_device_bytes", "ranges")]
+
+
 class SSQ:
     """the product's C-ABI (include/ssq.h); raises when libssq.so is missing — there is no fallback"""
     OPTS_WORDS = 30
@@ -110,6 +119,14 @@ class SSQ:
 
     def index_build(self, fasta, prefix=None, device=0):
         self.ck(self.lib.ssq_index_build(fasta.encode(), (prefix or fasta).encode(), C.c_int(device)), "ssq_index_build")
+
+    def index_build_ex(self, fasta, prefix=None, device=0, path=0, work_bytes=0):
+        """ssq_index_build_ex: path 0 auto, 2 device (multi-pass) sort, 3 host; work_bytes = the
+        multi-pass working budget (0: from free device memory).  Returns the stats as a dict ("path" = the path that ran)."""
+        opt = IndexBuildOpts(path, 0, work_bytes)
+        st = IndexBuildStats()
+        self.ck(self.lib.ssq_index_build_ex(fasta.encode(), (prefix or fasta).encode(), C.c_int(device), C.byref(opt), C.byref(st)), "ssq_index_build_ex")
+        return {k: getattr(st, k) for k, _ in IndexBuildStats._fields_ if k != "pad"}
 
     def index_free(self, h):
         self.lib.ssq_index_free(h)

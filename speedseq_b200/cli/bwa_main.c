@@ -531,7 +531,15 @@ static int main_index(int argc, char **argv)
 		else if (argv[i][0] != '-' && !fa) fa = argv[i];
 	}
 	if (!fa) { fprintf(stderr, "Usage: bwa index [-p prefix] <in.fasta>\n"); return 1; }
-	if ((rc = ssq_index_build(fa, prefix ? prefix : fa, device))) die("ssq_index_build", rc);
+	ssq_index_build_stats_t st;
+	static const char *const path_name[4] = {"", "", "device suffix sort", "host suffix sort"};
+	if ((rc = ssq_index_build_ex(fa, prefix ? prefix : fa, device, NULL, &st))) die("ssq_index_build_ex", rc);
+	if (st.path == 2)
+		fprintf(stderr, "[bwa_index] %s: %lld passes, %lld rounds, %.2f GB of device memory\n", path_name[2], (long long)st.passes, (long long)st.rounds, st.peak_device_bytes / 1e9);
+	else if (st.path == 3 && ssq_last_error()[0])
+		fprintf(stderr, "[bwa_index] %s: %s\n", path_name[3], ssq_last_error());
+	else
+		fprintf(stderr, "[bwa_index] %s\n", path_name[st.path & 3]);
 	return 0;
 }
 

@@ -6,13 +6,12 @@
 // Upstream routines replaced (not vendored in the reference tree): bns_fasta2bntseq, bwt_pac2bwt/bwt_bwtgen,
 // bwt_bwtupdate_core, bwt_cal_sa.
 //
-// Design: the text T = forward + reverse-complement strand never leaves its 2-bit packing; the suffix array of T$ is
-// built by prefix doubling where every round is one LSD radix sort of (rank[i], rank[i+h]) pairs over all suffixes
-// (CUB DeviceRadixSort — HBM-streaming plumbing), ranks are re-derived with a max-scan, and the loop stops when all ranks
-// are distinct (h doubles from 16, so ~log2(longest repeat/16) rounds).  BWT symbols, the occ checkpoints every 128
-// symbols and the SA samples every 32 rows are then gathered by streaming kernels and written in the reference's layout.
-// The device sort holds 2*l_pac + 1 < 2^31 suffixes (1.07 Gbp).  Beyond that (whole GRCh37: 6.2 G suffixes) the suffix array is
-// built on the host — induced sorting with 64-bit indices (ssq_sais.h), BWT / occ checkpoints / SA samples by host threads — and
+// Design: the text T = forward + reverse-complement strand never leaves its 2-bit packing; the suffix array of T$ is built
+// by the multi-pass device sort of ssq_sapass.cuh (5 B of HBM per suffix for the rank array + a working budget sized from the
+// device's free memory, fewer than 2^40 suffixes: whole GRCh37 has 6.2 G), and BWT symbols, the occ checkpoints every 128
+// symbols and the SA samples every 32 rows are written in the reference's layout.  Without a device or the memory for it, the
+// suffix array is built on the host — induced sorting with 64-bit indices (ssq_sais.h), BWT / occ checkpoints / SA samples by
+// host threads — and
 // written in the same layout; no GPU is touched on that path (SSQ_INDEX_HOST=1 forces it for any size: the CPU tests pin it on
 // the reference's goldens).  FASTA parsing and the lrand48() replacement of ambiguous bases are inherently sequential (the
 // random stream is consumed in file order) and run on the host.
@@ -28,8 +27,7 @@
 #include <thread>
 #include "ssq_host.h"
 #include "ssq_sais.h"
-
-#define CKB(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { ssq_set_error("%s:%d: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); rc = SSQ_ECUDA; goto done; } } while (0)
+#include "ssq_sapass.cuh"
 
 // ---------------------------------------------------------------------------- host: FASTA ----
 struct FaContig { std::string name, anno; i64 offset; i32 len, n_ambs; };
@@ -115,101 +113,17 @@ static int write_text_files(const char *prefix, const std::vector<FaContig> &ctg
 }
 
 // ------------------------------------------------------------------------------ kernels ----
-// symbol i of T (0 <= i < n = 2*l_pac) straight from the 2-bit forward strand
-__device__ __forceinline__ u32 tsym(const uint8_t *__restrict__ pac, i64 l_pac, i64 i)
+// one thread per element of [0, n) (grid-stride past 2^30 threads); f is one of the SSQ_HD bodies of ssq_sapass.cuh
+template <class F> __global__ void k_sp_each(u64 n, F f)
 {
-	if (i >= l_pac) { const i64 f = 2 * l_pac - 1 - i; return 3u - ((pac[f >> 2] >> ((~f & 3) << 1)) & 3u); }
-	return (pac[i >> 2] >> ((~i & 3) << 1)) & 3u;
+	for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (u64)gridDim.x * blockDim.x) f(j);
 }
-
-// round 0 key: 16 symbols (zero padded) then min(remaining,16); the sentinel suffix i==n gets the unique smallest key 0
-__global__ void k_ib_init(const uint8_t *__restrict__ pac, i64 l_pac, u32 n1, u64 *key, u32 *idx)
+template <class F> static cudaError_t sp_launch(u64 n, const F &f)
 {
-	const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n1) return;
-	const i64 n = 2 * l_pac;
-	u64 k = 0;
-	const i64 rem = n - i;
-	const int m = rem < 16 ? (int)rem : 16;
-	for (int j = 0; j < 16; ++j) k = k << 2 | (j < m ? tsym(pac, l_pac, (i64)i + j) : 0u);
-	key[i] = k << 8 | (u64)m;
-	idx[i] = i;
-}
-__global__ void k_ib_flags(u32 n1, const u64 *__restrict__ ks, u32 *head)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	if (j >= n1) return;
-	head[j] = (j == 0 || ks[j] != ks[j - 1]) ? j : 0u;
-}
-__global__ void k_ib_scatter_rank(u32 n1, const u32 *__restrict__ idx, const u32 *__restrict__ rank_sorted, u32 *rank)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	if (j < n1) rank[idx[j]] = rank_sorted[j];
-}
-__global__ void k_ib_count_heads(u32 n1, const u32 *__restrict__ rank_sorted, unsigned long long *n_groups)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	unsigned v = (j < n1 && rank_sorted[j] == j) ? 1u : 0u;
-	for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-	if ((threadIdx.x & 31) == 0 && v) atomicAdd(n_groups, (unsigned long long)v);
-}
-__global__ void k_ib_pairkey(u32 n1, u32 h, const u32 *__restrict__ idx, const u32 *__restrict__ rank, u64 *key)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	if (j >= n1) return;
-	const u32 i = idx[j];
-	const u64 second = (u64)i + h < (u64)n1 ? (u64)rank[i + h] + 1 : 0;
-	key[j] = (u64)rank[i] << 32 | second;
-}
-__global__ void k_ib_primary(u32 n1, const u32 *__restrict__ sa, u32 *primary)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	if (j < n1 && sa[j] == 0) *primary = j;
-}
-// BWT symbol stream without the '$' row, one byte per symbol
-__global__ void k_ib_bwtsym(const uint8_t *__restrict__ pac, i64 l_pac, u32 n, u32 primary, const u32 *__restrict__ sa, uint8_t *bs)
-{
-	const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
-	if (j >= n) return;
-	const u32 r = j + (j >= primary);
-	bs[j] = (uint8_t)tsym(pac, l_pac, (i64)sa[r] - 1);
-}
-// per 128-symbol block: the four symbol counts (for the checkpoint scan)
-__global__ void k_ib_blockcnt(u32 n, u32 n_blk, const uint8_t *__restrict__ bs, u64 *c0, u64 *c1, u64 *c2, u64 *c3)
-{
-	const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
-	if (b >= n_blk) return;
-	u32 c[4] = {0, 0, 0, 0};
-	const u32 lo = b * 128, hi = lo + 128 < n ? lo + 128 : n;
-	for (u32 j = lo; j < hi; ++j) ++c[bs[j]];
-	c0[b] = c[0]; c1[b] = c[1]; c2[b] = c[2]; c3[b] = c[3];
-}
-// interleaved layout: block b at words [16b, 16b+16) = u64 occ[4] then 8 symbol words (MSB first); trailing checkpoint after the last word
-__global__ void k_ib_interleave(u32 n, u32 n_blk, const uint8_t *__restrict__ bs, const u64 *__restrict__ c0, const u64 *__restrict__ c1,
-                                const u64 *__restrict__ c2, const u64 *__restrict__ c3, u32 *out, u64 total_words)
-{
-	const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
-	if (b > n_blk) return;
-	if (b == n_blk) { // final checkpoint: totals
-		u32 *o = out + total_words - 8; // only 4-byte aligned when the symbol-word count is odd
-		const u64 t[4] = {c0[n_blk], c1[n_blk], c2[n_blk], c3[n_blk]};
-		for (int c = 0; c < 4; ++c) { o[2 * c] = (u32)t[c]; o[2 * c + 1] = (u32)(t[c] >> 32); }
-		return;
-	}
-	u64 *o = (u64*)(out + (u64)b * 16);
-	o[0] = c0[b]; o[1] = c1[b]; o[2] = c2[b]; o[3] = c3[b];
-	for (u32 w = 0; w < 8; ++w) {
-		const u32 lo = b * 128 + w * 16;
-		if (lo >= n) break;
-		u32 v = 0;
-		for (u32 k = 0; k < 16; ++k) { const u32 j = lo + k; v = v << 2 | (j < n ? (u32)bs[j] : 0u); }
-		out[(u64)b * 16 + 8 + w] = v;
-	}
-}
-__global__ void k_ib_sasample(u32 n_sa, const u32 *__restrict__ sa, u64 *out)
-{
-	const u32 k = blockIdx.x * blockDim.x + threadIdx.x;
-	if (k >= 1 && k < n_sa) out[k - 1] = (u64)sa[(u64)k * 32];
+	if (!n) return cudaSuccess;
+	const u64 g = (n + 255) / 256;
+	k_sp_each<<<(unsigned)(g < (1u << 22) ? g : (1u << 22)), 256>>>(n, f);
+	return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------- host path ----
@@ -241,7 +155,7 @@ static int build_bwt_sa_host_impl(const char *prefix, const std::vector<uint8_t>
 		for (int t = 0; t < n_thr; ++t) { const u64 lo = per * t, hi = lo + per < total ? lo + per : total; if (lo < hi) th.emplace_back(fn, lo, hi); }
 		for (auto &x : th) x.join();
 	};
-	// T$ over {0: '$', 1..4: A C G T}: forward strand then its reverse complement (tsym on the device path)
+	// T$ over {0: '$', 1..4: A C G T}: forward strand then its reverse complement (sp_sym on the device paths)
 	par(n, [&](u64 lo, u64 hi) {
 		for (u64 i = lo; i < hi; ++i) {
 			const bool fw = i < (u64)l_pac;
@@ -303,104 +217,129 @@ static int build_bwt_sa_host_impl(const char *prefix, const std::vector<uint8_t>
 	return SSQ_OK;
 }
 
+// -------------------------------------------------------------------- multi-pass device path ----
+// the backend sp_build (ssq_sapass.cuh) runs on: kernels over the SSQ_HD bodies, CUB for sorts and scans
+struct SpDevice {
+	u64 cur = 0, peak = 0;
+	SpBuf tmp = {0, 0};
+	~SpDevice() { release(tmp); }
+	int ck(cudaError_t e) { if (e == cudaSuccess) return 0; ssq_set_error("multi-pass index build: %s", cudaGetErrorString(e)); return SSQ_ECUDA; }
+	int need(SpBuf &b, u64 bytes)
+	{
+		if (bytes <= b.cap) return 0;
+		release(b);
+		if (cudaMalloc(&b.p, bytes) != cudaSuccess) {
+			cudaGetLastError();
+			size_t fr = 0, tot = 0;
+			cudaMemGetInfo(&fr, &tot);
+			b.p = 0;
+			ssq_set_error("multi-pass index build: cannot allocate %.3f GB of device memory (this build holds %.3f GB, %.3f GB free)", bytes / 1e9, cur / 1e9, fr / 1e9);
+			return SSQ_ENOMEM;
+		}
+		b.cap = bytes; cur += bytes;
+		if (cur > peak) peak = cur;
+		return 0;
+	}
+	void release(SpBuf &b) { if (b.p) { cudaFree(b.p); cur -= b.cap; } b.p = 0; b.cap = 0; }
+	int put(void *d, const void *h, u64 bytes) { return ck(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice)); }
+	int get(void *h, const void *d, u64 bytes) { return ck(cudaMemcpy(h, d, bytes, cudaMemcpyDeviceToHost)); }
+	int zero(void *d, u64 bytes) { return ck(cudaMemset(d, 0, bytes)); }
+	template <class F> int each(u64 n, const F &f) { return ck(sp_launch(n, f)); }
+	int sort(u64 *&k, u64 *&v, u64 *&k2, u64 *&v2, u64 m, int bits)
+	{
+		cub::DoubleBuffer<u64> kb(k, k2), vb(v, v2);
+		size_t tb = 0;
+		int rc;
+		if ((rc = ck(cub::DeviceRadixSort::SortPairs(0, tb, kb, vb, (int)m, 0, bits)))) return rc;
+		if ((rc = need(tmp, tb + 1))) return rc;
+		if ((rc = ck(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kb, vb, (int)m, 0, bits)))) return rc;
+		k = kb.Current(); k2 = kb.Alternate(); v = vb.Current(); v2 = vb.Alternate();
+		return 0;
+	}
+	int max_scan(u64 *a, u64 m)
+	{
+		size_t tb = 0;
+		int rc;
+		if ((rc = ck(cub::DeviceScan::InclusiveScan(0, tb, a, a, cub::Max(), (int)m)))) return rc;
+		if ((rc = need(tmp, tb + 1))) return rc;
+		return ck(cub::DeviceScan::InclusiveScan(tmp.p, tb, a, a, cub::Max(), (int)m));
+	}
+	int excl_sum(u64 *a, u64 m)
+	{
+		size_t tb = 0;
+		int rc;
+		if ((rc = ck(cub::DeviceScan::ExclusiveSum(0, tb, a, a, (int)m)))) return rc;
+		if ((rc = need(tmp, tb + 1))) return rc;
+		return ck(cub::DeviceScan::ExclusiveSum(tmp.p, tb, a, a, (int)m));
+	}
+};
+
 // -------------------------------------------------------------------------------- driver ----
-extern "C" int ssq_index_build(const char *fasta, const char *prefix, int device)
+#define SP_MARGIN(fr) ((u64)(1ull << 30) + (u64)(fr) / 32) // device memory left to other users of the card
+// the least working budget the automatic choice takes the device with: 256 MB, and at least enough for 32 first-sort passes
+static u64 sp_min_work(u64 n1) { const u64 w = n1 * SP_PASS_ROW_BYTES / 32; return w > (256ull << 20) ? w : (256ull << 20); }
+
+extern "C" int ssq_index_build_ex(const char *fasta, const char *prefix, int device, const ssq_index_build_opts_t *opt, ssq_index_build_stats_t *st)
 {
 	if (!fasta) return SSQ_EINVAL;
 	if (!prefix) prefix = fasta;
+	ssq_index_build_stats_t st0;
+	if (!st) st = &st0;
+	memset(st, 0, sizeof *st);
+	const int want = opt ? opt->path : 0;
+	if (want != 0 && want != 2 && want != 3) { ssq_set_error("index build path %d: 0 auto, 2 device (multi-pass) sort, 3 host", want); return SSQ_EINVAL; }
 	int rc;
 	std::vector<FaContig> ctg; std::vector<FaHole> holes; std::vector<uint8_t> pac;
 	i64 l_pac = 0;
 	if ((rc = parse_fasta(fasta, ctg, holes, pac, l_pac))) { ssq_set_error("cannot read any sequence from %s", fasta); return rc; }
 	pac.resize((size_t)(l_pac >> 2) + 2, 0);
-	const i64 n64 = 2 * l_pac;
+	const u64 n1 = 2 * (u64)l_pac + 1;
+	const bool small = n1 < 0x7fffffffull; // 32-bit suffix-array entries suffice on the host path
+	const u64 fixed = 5 * n1 + pac.size() + SP_NBUCKET * 8 + 64; // rank planes, text, bucket counts
 	const char *force = getenv("SSQ_INDEX_HOST"); // 1: host path with the narrowest entry type that fits, 40 / 64: with 40- / 64-bit entries
-	if (n64 + 1 >= 0x7fffffffLL || (force && atoi(force))) { // beyond the device sort of this build (or asked for): everything on the host, no GPU needed
-		if ((rc = write_text_files(prefix, ctg, holes, pac, l_pac))) { ssq_set_error("cannot write %s.{ann,amb,pac}", prefix); return rc; }
-		const int f = force ? atoi(force) : 0; // entry width: what was asked for, else 32 bits while they suffice, else 40 (5 bytes per suffix)
-		return build_bwt_sa_host(prefix, pac, l_pac, f == 64 ? 64 : (f == 40 || n64 + 1 >= 0x7fffffffLL) ? 40 : 32);
-	}
-	if ((rc = ssq_use_device(device))) return rc;
-	if ((rc = write_text_files(prefix, ctg, holes, pac, l_pac))) { ssq_set_error("cannot write %s.{ann,amb,pac}", prefix); return rc; }
-	const u32 n = (u32)n64, n1 = n + 1;
-	const unsigned G1 = (n1 + 255) / 256;
-	uint8_t *d_pac = 0, *d_bs = 0;
-	u64 *d_key[2] = {0, 0}, *d_cnt[4] = {0, 0, 0, 0}, *d_cnts[4] = {0, 0, 0, 0}, *d_sas = 0;
-	u32 *d_idx[2] = {0, 0}, *d_rank = 0, *d_head = 0, *d_misc = 0, *d_out = 0;
-	void *d_tmp = 0;
-	size_t tmp_bytes = 0, tb;
-	unsigned long long n_groups = 0;
-	u32 primary = 0;
-	u64 L2[5] = {0, 0, 0, 0, 0};
-	const u32 n_blk = (n + 127) / 128;
-	const u64 raw_words = ((u64)n + 15) / 16, total_words = raw_words + ((u64)n_blk + 1) * 8;
-	const u32 n_sa = (u32)(((u64)n + 32) / 32);
-	std::vector<uint8_t> h_out;
-	FILE *fp = 0;
-	cub::DoubleBuffer<u64> kb; cub::DoubleBuffer<u32> vb;
-	CKB(cudaMalloc(&d_pac, pac.size()));
-	CKB(cudaMemcpy(d_pac, pac.data(), pac.size(), cudaMemcpyHostToDevice));
-	for (int i = 0; i < 2; ++i) { CKB(cudaMalloc(&d_key[i], (size_t)n1 * 8)); CKB(cudaMalloc(&d_idx[i], (size_t)n1 * 4)); }
-	CKB(cudaMalloc(&d_rank, (size_t)n1 * 4)); CKB(cudaMalloc(&d_head, (size_t)n1 * 4)); CKB(cudaMalloc(&d_misc, 64));
-	kb = cub::DoubleBuffer<u64>(d_key[0], d_key[1]); vb = cub::DoubleBuffer<u32>(d_idx[0], d_idx[1]);
-	cub::DeviceRadixSort::SortPairs(0, tmp_bytes, kb, vb, (int)n1, 0, 64);
-	tb = 0; cub::DeviceScan::InclusiveScan(0, tb, d_head, d_head, cub::Max(), (int)n1); if (tb > tmp_bytes) tmp_bytes = tb;
-	tb = 0; cub::DeviceScan::ExclusiveSum(0, tb, (u64*)0, (u64*)0, (int)n_blk + 1); if (tb > tmp_bytes) tmp_bytes = tb;
-	CKB(cudaMalloc(&d_tmp, tmp_bytes));
-	// round 0: 16-mer keys
-	k_ib_init<<<G1, 256>>>(d_pac, l_pac, n1, kb.Current(), vb.Current());
-	CKB(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, kb, vb, (int)n1, 0, 40));
-	for (u32 h = 16;; h <<= 1) {
-		// ranks = position of the head of each run of equal keys
-		k_ib_flags<<<G1, 256>>>(n1, kb.Current(), d_head);
-		CKB(cub::DeviceScan::InclusiveScan(d_tmp, tmp_bytes, d_head, d_head, cub::Max(), (int)n1));
-		k_ib_scatter_rank<<<G1, 256>>>(n1, vb.Current(), d_head, d_rank);
-		CKB(cudaMemset(d_misc, 0, 16));
-		k_ib_count_heads<<<G1, 256>>>(n1, d_head, (unsigned long long*)d_misc);
-		CKB(cudaMemcpy(&n_groups, d_misc, 8, cudaMemcpyDeviceToHost));
-		if (n_groups == n1) break;
-		if (h >= n1) { ssq_set_error("suffix sort did not converge"); rc = SSQ_ECUDA; goto done; }
-		k_ib_pairkey<<<G1, 256>>>(n1, h, vb.Current(), d_rank, kb.Current());
-		CKB(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, kb, vb, (int)n1, 0, 64));
-	}
-	{
-		const u32 *d_sa = vb.Current(); // SA of T$ (n+1 rows)
-		k_ib_primary<<<G1, 256>>>(n1, d_sa, d_misc + 4);
-		CKB(cudaMemcpy(&primary, d_misc + 4, 4, cudaMemcpyDeviceToHost));
-		CKB(cudaMalloc(&d_bs, (size_t)n + 16));
-		k_ib_bwtsym<<<(n + 255) / 256, 256>>>(d_pac, l_pac, n, primary, d_sa, d_bs);
-		for (int c = 0; c < 4; ++c) { CKB(cudaMalloc(&d_cnt[c], ((size_t)n_blk + 2) * 8)); CKB(cudaMalloc(&d_cnts[c], ((size_t)n_blk + 2) * 8)); CKB(cudaMemset(d_cnt[c], 0, ((size_t)n_blk + 2) * 8)); }
-		k_ib_blockcnt<<<(n_blk + 255) / 256, 256>>>(n, n_blk, d_bs, d_cnt[0], d_cnt[1], d_cnt[2], d_cnt[3]);
-		for (int c = 0; c < 4; ++c) CKB(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_cnt[c], d_cnts[c], (int)n_blk + 1));
-		for (int c = 0; c < 4; ++c) CKB(cudaMemcpy(&L2[c + 1], d_cnts[c] + n_blk, 8, cudaMemcpyDeviceToHost));
-		for (int c = 2; c <= 4; ++c) L2[c] += L2[c - 1];
-		CKB(cudaMalloc(&d_out, total_words * 4));
-		CKB(cudaMemset(d_out, 0, total_words * 4));
-		k_ib_interleave<<<(n_blk + 1 + 255) / 256, 256>>>(n, n_blk, d_bs, d_cnts[0], d_cnts[1], d_cnts[2], d_cnts[3], d_out, total_words);
-		CKB(cudaGetLastError());
-		h_out.resize(total_words * 4);
-		CKB(cudaMemcpy(h_out.data(), d_out, total_words * 4, cudaMemcpyDeviceToHost));
-		{
-			std::string p(prefix);
-			const u64 prim64 = primary;
-			if (!(fp = fopen((p + ".bwt").c_str(), "wb"))) { ssq_set_error("cannot write %s.bwt", prefix); rc = SSQ_EIO; goto done; }
-			fwrite(&prim64, 8, 1, fp); fwrite(L2 + 1, 8, 4, fp); fwrite(h_out.data(), 1, h_out.size(), fp);
-			fclose(fp); fp = 0;
-			CKB(cudaMalloc(&d_sas, (size_t)n_sa * 8));
-			k_ib_sasample<<<(n_sa + 255) / 256, 256>>>(n_sa, d_sa, d_sas);
-			h_out.resize((size_t)(n_sa - 1) * 8);
-			CKB(cudaMemcpy(h_out.data(), d_sas, (size_t)(n_sa - 1) * 8, cudaMemcpyDeviceToHost));
-			if (!(fp = fopen((p + ".sa").c_str(), "wb"))) { ssq_set_error("cannot write %s.sa", prefix); rc = SSQ_EIO; goto done; }
-			const u64 sa_intv = 32, seq_len = n;
-			fwrite(&prim64, 8, 1, fp); fwrite(L2 + 1, 8, 4, fp); fwrite(&sa_intv, 8, 1, fp); fwrite(&seq_len, 8, 1, fp);
-			fwrite(h_out.data(), 1, h_out.size(), fp);
-			fclose(fp); fp = 0;
+	int path = want;
+	u64 work = opt ? opt->work_bytes : 0;
+	char why[256] = "";
+	if (want == 0 && force && atoi(force)) path = 3;
+	if (path == 2 && n1 >= SP_MAX_N1) { ssq_set_error("%llu suffixes: the device sort holds fewer than 2^40", (unsigned long long)n1); return SSQ_EINVAL; }
+	if (path != 3) {
+		if ((rc = ssq_use_device(device))) {
+			if (path != 0 || small) return rc;
+			path = 3; // a reference past 2^31 suffixes and no usable device: the host path, no GPU needed
+			snprintf(why, sizeof why, "no usable CUDA device");
+		} else {
+			size_t fr = 0, tot = 0;
+			cudaError_t e = cudaMemGetInfo(&fr, &tot);
+			if (e != cudaSuccess) { ssq_set_error("cudaMemGetInfo: %s", cudaGetErrorString(e)); return SSQ_ECUDA; }
+			const u64 avail = (u64)fr > SP_MARGIN(fr) ? (u64)fr - SP_MARGIN(fr) : 0;
+			if (!work) work = avail > fixed ? avail - fixed : 0;
+			if (path == 0) {
+				if (n1 < SP_MAX_N1 && work >= sp_min_work(n1)) path = 2;
+				else {
+					path = 3;
+					snprintf(why, sizeof why, "%.1f GB of device memory free; the device sort needs %.1f GB for its rank array and text + %.1f GB to work in",
+					         fr / 1e9, (fixed + SP_MARGIN(fr)) / 1e9, sp_min_work(n1) / 1e9);
+				}
+			} else if (!work) {
+				ssq_set_error("device index build: %.1f GB of device memory free, %.1f GB needed for the rank array and text before any working space",
+				              fr / 1e9, (fixed + SP_MARGIN(fr)) / 1e9);
+				return SSQ_ENOMEM;
+			}
 		}
 	}
-done:
-	if (fp) fclose(fp);
-	cudaFree(d_pac); cudaFree(d_bs); cudaFree(d_rank); cudaFree(d_head); cudaFree(d_misc); cudaFree(d_out); cudaFree(d_tmp); cudaFree(d_sas);
-	for (int i = 0; i < 2; ++i) { cudaFree(d_key[i]); cudaFree(d_idx[i]); }
-	for (int c = 0; c < 4; ++c) { cudaFree(d_cnt[c]); cudaFree(d_cnts[c]); }
+	st->path = path;
+	if ((rc = write_text_files(prefix, ctg, holes, pac, l_pac))) { ssq_set_error("cannot write %s.{ann,amb,pac}", prefix); return rc; }
+	if (path == 2) {
+		SpDevice be;
+		return sp_build(be, pac.data(), pac.size(), l_pac, prefix, work, st);
+	}
+	const int f = force ? atoi(force) : 0; // entry width: what was asked for, else 32 bits while they suffice, else 40 (5 bytes per suffix)
+	rc = build_bwt_sa_host(prefix, pac, l_pac, f == 64 ? 64 : (f == 40 || !small) ? 40 : 32);
+	if (!rc) ssq_set_error("%s", why); // why the automatic choice took the host path (empty when it was asked for)
 	return rc;
+}
+
+extern "C" int ssq_index_build(const char *fasta, const char *prefix, int device)
+{
+	return ssq_index_build_ex(fasta, prefix, device, 0, 0);
 }

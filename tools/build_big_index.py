@@ -1,13 +1,22 @@
 #!/usr/bin/env python
-"""`ssq_index_build` on a reference beyond the device sort's limit (2^31 - 2 suffixes): the host path (64-bit induced sorting,
-csrc/ssq_sais.h).  Builds a seeded synthetic genome (8 contigs, planted repeat family; default 2.2 Gbp = 4.4 G suffixes, more BWT
-rows than 2^32; 3100000000 = the size of GRCh37), indexes it without touching a GPU, then checks the result three ways:
+"""`ssq_index_build_ex` on a large reference, on the path(s) asked for, then three checks of the result.  Builds a seeded
+synthetic genome (8 contigs, planted repeat family; default 2.2 Gbp = 4.4 G suffixes, more BWT rows than 2^32; 3100000000 = the
+size of GRCh37), indexes it, then checks:
   * header: primary row, cumulative base counts = the base composition of forward + reverse-complement strand;
   * order: a million random pairs of consecutive SA samples (32 rows apart) are in lexicographic order, compared on the text;
   * function: the CPU oracle loads the index and places simulated read pairs at their origins.
-usage: build_big_index.py [genome_bp] [n_pairs]      (about 15 bytes of host memory per reference base pair)"""
+--path: passes (device sort), host, auto, both (= passes,host) or a comma list; the first path builds the index that is
+checked (always afresh: index files left in the cache are removed first), every further one builds into its own prefix and must
+give the same five files byte for byte.  Each build prints the path that ran (from the stats), its wall time, the device sort's
+stats and this process's peak host memory so far.
+--repeats: hard repeats on top of the generator's diverged family: 5 % of the genome as exact copies of 10-100 kb segments and
+1 % as 171 bp satellite arrays at 2 % divergence, so that many suffixes stay tied for many doubling rounds.
+usage: build_big_index.py [genome_bp] [n_pairs] [--path P] [--repeats]    (host path: about 15 bytes of host memory per bp)"""
+import argparse
 import ctypes as C
+import filecmp
 import os
+import resource
 import struct
 import subprocess
 import sys
@@ -19,23 +28,89 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import bench
+from speedseq_b200 import capi
 
-glen = int(sys.argv[1]) if len(sys.argv) > 1 else 2_200_000_000
-n_pairs = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
-cache = bench.cache_dir()
-lib = C.CDLL(os.path.join(ROOT, "speedseq_b200", "libssq.so"))
-lib.ssq_index_build.argtypes = [C.c_char_p, C.c_char_p, C.c_int]
-lib.ssq_last_error.restype = C.c_char_p
+ap = argparse.ArgumentParser()
+ap.add_argument("genome_bp", nargs="?", type=int, default=2_200_000_000)
+ap.add_argument("n_pairs", nargs="?", type=int, default=2000)
+ap.add_argument("--path", default="passes")
+ap.add_argument("--repeats", action="store_true")
+args = ap.parse_args()
+glen, n_pairs = args.genome_bp, args.n_pairs
+PATHS = {"auto": 0, "passes": 2, "host": 3}
+NAMES = {2: "device suffix sort", 3: "host suffix sort"}
+paths = ["passes", "host"] if args.path == "both" else args.path.split(",")
+cache = os.path.join(bench.cache_dir(), "hard") if args.repeats else bench.cache_dir()
+ssq = capi.SSQ()
+PLANTED = []  # [start, end) of every planted copy, source and target: a read from one of them has no unique origin
+
+
+def plant(n, seed, g=None):
+    """the hard repeats of --repeats (seeded): copies into g when given, their intervals into PLANTED either way"""
+    PLANTED.clear()
+    rng = np.random.default_rng(seed + 1000)
+    done = 0
+    while done < 0.05 * n:
+        L = int(rng.integers(10000, 100001))
+        a, b = (int(x) for x in rng.integers(0, n - L, 2))
+        if g is not None:
+            g[b:b + L] = g[a:a + L]
+        PLANTED.extend([(a, a + L), (b, b + L)])
+        done += L
+    unit = rng.integers(0, 4, 171).astype(np.uint8)
+    done = 0
+    while done < 0.01 * n:
+        k = int(rng.integers(5, 60))
+        arr = np.tile(unit, k)
+        m = rng.random(arr.size) < 0.02
+        arr[m] = rng.integers(0, 4, int(m.sum())).astype(np.uint8)
+        b = int(rng.integers(0, n - arr.size))
+        if g is not None:
+            g[b:b + arr.size] = arr
+        PLANTED.append((b, b + arr.size))
+        done += arr.size
+
+
+if args.repeats:  # the same generator, hard repeats planted on top
+    _synth = bench.synth_genome
+
+    def hard(n, seed, repeat_frac=0.08):
+        g = _synth(n, seed, repeat_frac)
+        plant(n, seed, g)
+        return g
+    bench.synth_genome = hard
+
+
+def build_one(fa, prefix, name):
+    t0 = time.time()
+    st = ssq.index_build_ex(fa, prefix, 0, path=PATHS[name])
+    dt = time.time() - t0
+    extra = ""
+    if st["path"] == 2:
+        extra = ": %d passes, %d rounds, %d chunks, %d suffixes open after the first sort (%.3f %%), largest group %d, %d oversize, %d finalisation ranges, peak %.1f GB of device memory" % (
+            st["passes"], st["rounds"], st["chunks"], st["unresolved_first"], 100.0 * st["unresolved_first"] / (2 * glen + 1), st["largest_group"], st["oversize_groups"], st["ranges"], st["peak_device_bytes"] / 1e9)
+    extra += "; peak host RSS of this process so far %.1f GB" % (resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 1e6)
+    print("ssq_index_build_ex --path %s -> %s: %.1f s for %d bp = %d suffixes%s" % (name, NAMES[st["path"]], dt, glen, 2 * glen + 1, extra), flush=True)
+    return dt
 
 
 def builder(fa):
-    t0 = time.time()
-    rc = lib.ssq_index_build(fa.encode(), None, 0)
-    assert rc == 0, lib.ssq_last_error()
-    print("ssq_index_build (host path): %.1f s for %d bp = %d suffixes" % (time.time() - t0, glen, 2 * glen + 1), flush=True)
+    build_one(fa, fa, paths[0])
 
 
+for ext in (".bwt", ".sa", ".pac", ".ann", ".amb"):  # the first path always builds: no check may run on an index some earlier run made
+    if os.path.exists(os.path.join(cache, "syn_%d.fa%s" % (glen, ext))):
+        os.remove(os.path.join(cache, "syn_%d.fa%s" % (glen, ext)))
 fa, g = bench.ensure_reference(cache, glen, builder)
+if args.repeats and not PLANTED:  # genome taken from the cache: the same seeded intervals
+    plant(glen, 20)
+for name in paths[1:]:
+    pre = fa + "." + name
+    build_one(fa, pre, name)
+    for ext in ("amb", "ann", "pac", "bwt", "sa"):
+        assert filecmp.cmp(fa + "." + ext, pre + "." + ext, shallow=False), "%s: .%s differs from --path %s" % (name, ext, paths[0])
+        os.remove(pre + "." + ext)
+    print("--path %s: all five files byte-identical to --path %s" % (name, paths[0]), flush=True)
 n = 2 * glen
 # --- header
 with open(fa + ".bwt", "rb") as f:
@@ -82,7 +157,15 @@ print("1,000,000 random pairs of consecutive SA samples are in lexicographic ord
 # --- function: the oracle aligns reads simulated from known positions
 import ssq_testlib as T
 rl = 150
-pos = rng.integers(0, glen - 1000, n_pairs)
+pos = rng.integers(0, glen - 1000, 4 * n_pairs)
+if PLANTED:  # only reads with a unique origin can be checked for placement
+    iv = np.array(sorted(PLANTED), np.int64)
+    reach = np.maximum.accumulate(iv[:, 1])
+    k = np.searchsorted(iv[:, 0], pos + 400, side="left")  # planted intervals starting before the fragment ends
+    hit = (k > 0) & (reach[np.maximum(k - 1, 0)] > pos)
+    print("%d of %d drawn fragments overlap planted copies and are not used" % (int(hit[:n_pairs].sum()), n_pairs), flush=True)
+    pos = pos[~hit]
+pos = pos[:n_pairs]
 bounds = np.linspace(0, glen, 9).astype(np.int64)
 fq = os.path.join(cache, "big_check.fq")
 acgt = np.frombuffer(b"ACGT", np.uint8)
