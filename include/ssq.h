@@ -342,6 +342,30 @@ int ssq_gunzip_inflate_dev(ssq_gunzip_t *g, const void *d_in, size_t n, void *d_
 int ssq_gunzip_stats(const ssq_gunzip_t *g, int64_t out[4]);
 void *ssq_gunzip_stream(ssq_gunzip_t *g);           /* cudaStream_t of the object, for event timing */
 void ssq_gunzip_free(ssq_gunzip_t *g);
+/* samblaster over name-grouped SAM text on the device (csrc/ssq_sbtext.cu): what the `samblaster` shim does with SAM it did not get
+ * from the fused stage (`speedseq realign`, the default config, any other aligner's output).  The same decision routines as the
+ * fused stage (ssq_dev3.cuh sb_*), first-seen-wins duplicate marking against the object's dup-set, and the three streams as text:
+ * FLAG re-printed in decimal with 0x400 on duplicates, MC:Z / MQ:i (the mate's CIGAR and MAPQ fields, verbatim) appended when
+ * absent, splitter QNAMEs suffixed _1 / _2, --removeDups / --excludeDups applied.  Only '\n' ends a line ('\r' stays in the last
+ * field); a last line without '\n' is taken when final.
+ * header: the SAM header text; its @SQ lines define the contig ids (first SN wins) and samblaster's padded offsets (LN + 2*500 + 1
+ * each).  One object = one run; one host thread at a time.  Without a usable GPU create returns SSQ_ENOGPU. */
+typedef struct ssq_sbtext ssq_sbtext_t;
+typedef struct {
+	const char *text[3]; size_t len[3];   /* 0 main records, 1 splitters, 2 discordants; pinned, owned by the object, valid until its next run */
+	uint64_t n_ids, n_dup, n_disc_lines, n_split_lines; /* QNAME blocks taken / marked duplicate; lines written to streams 2 and 1 */
+} ssq_sbtext_out_t;
+int ssq_sbtext_create(int device, const ssq_sb_opts_t *sb, const char *header, size_t header_len, ssq_sbtext_t **out);
+/* text[0, len): record lines from a line start on (len < 2^31); final: nothing follows.  Processes whole QNAME blocks, at most
+ * max_blocks of them (0 = no limit); the last block is held back unless final (the next line may continue it); *used = bytes
+ * consumed (0 when no whole block is in the text yet: call again with more).  SSQ_EFORMAT: a line in the range the device does
+ * not take — fewer than 11 fields, a NUL byte, FLAG or POS not plain digits, a CIGAR the parser does not fully consume, an RNAME
+ * other than `*` not in @SQ, a QNAME block over 256 lines, a mapped primary line with RNAME `*`; nothing is consumed and
+ * ssq_last_error() names the line (the caller runs its host code over these lines, marking through ssq_sbtext_dupset). */
+int ssq_sbtext_run(ssq_sbtext_t *s, const char *text, size_t len, int final, uint64_t max_blocks, size_t *used, ssq_sbtext_out_t *out);
+ssq_dupset_t *ssq_sbtext_dupset(ssq_sbtext_t *s);   /* the set it marks against, so that a host fallback can share it */
+void *ssq_sbtext_stream(ssq_sbtext_t *s);           /* cudaStream_t of the object, for event timing */
+void ssq_sbtext_free(ssq_sbtext_t *s);
 /* the sorted runs of consecutive batches -> one sorted record stream (stable: equal keys keep batch order); free with ssq_free */
 int ssq_bam_merge_runs(int n_runs, const void *const *runs, const size_t *lens, void **out, size_t *out_len);
 

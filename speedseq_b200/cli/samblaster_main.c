@@ -10,6 +10,9 @@
  * ssq_dupset_mark() (radix sort + adjacent-equal mark within the chunk, binary search against the device-resident sorted
  * set of earlier signatures, SURVEY.md §8a a17).  Parsing, MC/MQ tags and the discordant / splitter predicates are text
  * bookkeeping done here.  Behaviour restated from samblaster 0.1.2x (not vendored in the reference tree; SURVEY Appendix B).
+ * Built with SSQ_SB_DEVICE_TEXT (the Makefile's ../bin/samblaster) the records after the header go through ssq_sbtext_run
+ * instead — parsing, decisions, marking and the three streams' text on the device — and this host code only takes over the runs
+ * of blocks the device refuses, marking against the same dup-set.
  */
 #define _GNU_SOURCE
 #include <stdio.h>
@@ -253,6 +256,10 @@ int main(int argc, char **argv)
 	uint8_t *dups = (uint8_t*)malloc(CHUNK_BLOCKS), *meta = (uint8_t*)malloc(CHUNK_BLOCKS);
 	int n_blocks = 0;
 	ssq_dupset_t *set = 0;
+#ifdef SSQ_SB_DEVICE_TEXT
+	char *hdr = 0;
+	size_t hdr_len = 0, hdr_cap = 0;
+#endif
 	memset(&o, 0, sizeof o); memset(&cur, 0, sizeof cur);
 	o.maxSplitCount = 2; o.minNonOverlap = 20; o.minIndelSize = 50; o.maxUnmappedBases = 50; o.out = stdout;
 	for (i = 1; i < argc; ++i) {
@@ -342,6 +349,10 @@ int main(int argc, char **argv)
 				}
 			}
 			fputs(line, o.out); if (o.disc) fputs(line, o.disc); if (o.split) fputs(line, o.split);
+#ifdef SSQ_SB_DEVICE_TEXT
+			if (hdr_len + (size_t)len > hdr_cap) { hdr_cap = (hdr_len + (size_t)len) * 2; hdr = (char*)realloc(hdr, hdr_cap); }
+			memcpy(hdr + hdr_len, line, (size_t)len); hdr_len += (size_t)len;
+#endif
 			continue;
 		}
 		if (!hdr_done) {
@@ -349,6 +360,81 @@ int main(int argc, char **argv)
 			for (i = 0; i < 3; ++i) if (fps[i]) fprintf(fps[i], "@PG\tID:SAMBLASTER\tVN:%s\tCL:%s\n", SB_VERSION, cl);
 			hdr_done = 1;
 		}
+#ifdef SSQ_SB_DEVICE_TEXT
+		{	/* the records from this line on: samblaster's stage on the device (ssq_sbtext_run) over large chunks of stdin.  A chunk
+			 * with lines the device does not take goes through the host code below, marking against the same dup-set, so "first
+			 * seen wins" spans both; the next chunk goes back to the device. */
+			ssq_sb_opts_t so;
+			ssq_sbtext_t *sbt = 0;
+			ssq_sbtext_out_t so_out;
+			size_t cap = 64 << 20, n = 0, at = 0, used;
+			char *buf;
+			int eof = 0, need = 0;
+			unsigned long long n_host = 0, n_host_blocks = 0;
+			char host_why[600] = "";
+			so.enabled = 1; so.exclude_dups = o.excludeDups; so.add_mate_tags = o.addMateTags; so.max_split_count = o.maxSplitCount; so.min_non_overlap = o.minNonOverlap;
+			so.min_indel_size = o.minIndelSize; so.max_unmapped_bases = o.maxUnmappedBases; so.remove_dups = o.removeDups; so.want_split = o.split != 0; so.want_disc = o.disc != 0;
+			if ((rc = ssq_sbtext_create(device, &so, hdr, hdr_len, &sbt))) { fprintf(stderr, "samblaster: %s\n", ssq_last_error()); return 1; }
+			set = ssq_sbtext_dupset(sbt);
+			while ((size_t)len > cap) cap *= 2;
+			if (!(buf = (char*)ssq_host_alloc(cap))) { fprintf(stderr, "samblaster: out of pinned host memory\n"); return 1; }
+			memcpy(buf, line, (size_t)len); n = (size_t)len;
+			for (;;) {
+				if (!eof && (need || n - at < cap / 2)) {
+					if (need && at == 0 && n == cap) { /* one block does not fit: a larger buffer */
+						char *b2 = (char*)ssq_host_alloc(cap * 2);
+						if (!b2) { fprintf(stderr, "samblaster: out of pinned host memory\n"); return 1; }
+						memcpy(b2, buf, n); ssq_host_free(buf); buf = b2; cap *= 2;
+					}
+					if (at) { memmove(buf, buf + at, n - at); n -= at; at = 0; }
+					n += fread(buf + n, 1, cap - n, stdin);
+					if (n < cap) eof = 1;
+					need = 0;
+				}
+				if (at == n && eof) break;
+				rc = ssq_sbtext_run(sbt, buf + at, n - at, eof, (uint64_t)CHUNK_BLOCKS, &used, &so_out);
+				if (rc == SSQ_OK) {
+					FILE *fps[3] = {o.out, o.split, o.disc};
+					for (i = 0; i < 3; ++i) if (fps[i] && so_out.len[i] && fwrite(so_out.text[i], 1, so_out.len[i], fps[i]) != so_out.len[i]) { fprintf(stderr, "samblaster: write failed\n"); return 1; }
+					o.n_ids += so_out.n_ids; o.n_dup += so_out.n_dup; o.n_disc += so_out.n_disc_lines; o.n_split += so_out.n_split_lines;
+					at += used;
+					if (!used) need = 1;
+				} else if (rc == SSQ_EFORMAT) { /* the blocks this run would have taken go through the host code; an unfinished last block waits */
+					size_t p = at, cur_at = at;
+					long long closed = 0;
+					const unsigned long long ids0 = o.n_ids;
+					if (!n_host++) snprintf(host_why, sizeof host_why, "%s", ssq_last_error());
+					while (p < n) {
+						const char *e = (const char*)memchr(buf + p, '\n', n - p);
+						const size_t q = e ? (size_t)(e - buf) + 1 : n;
+						char *s;
+						line_t l;
+						if (!e && !eof) break;
+						s = (char*)malloc(q - p + 1); memcpy(s, buf + p, q - p); s[q - p] = 0;
+						parse_line(&l, s);
+						if (cur.n && strcmp(cur.lines[0].f[0], l.f[0]) != 0) {
+							CLOSE_BLOCK();
+							if (++closed == CHUNK_BLOCKS) { free(l.text); free(l.f); break; }
+						}
+						if (!cur.n) cur_at = p;
+						if (cur.n == cur.m) { cur.m = cur.m ? cur.m * 2 : 4; cur.lines = (line_t*)realloc(cur.lines, sizeof(line_t) * cur.m); }
+						cur.lines[cur.n++] = l;
+						p = q;
+					}
+					if (closed == CHUNK_BLOCKS) at = p;
+					else if (eof) { CLOSE_BLOCK(); at = n; }
+					else { free_block(&cur); memset(&cur, 0, sizeof cur); at = cur_at; }
+					FLUSH_CHUNK();
+					n_host_blocks += o.n_ids - ids0;
+				} else { fprintf(stderr, "samblaster: ssq_sbtext_run failed (%d): %s\n", rc, ssq_last_error()); return 1; }
+			}
+			if (n_host) fprintf(stderr, "samblaster: %llu QNAME blocks went through the host code (%llu chunks; the first: %s)\n", n_host_blocks, n_host, host_why);
+			ssq_host_free(buf);
+			ssq_sbtext_free(sbt); /* frees the dup-set too */
+			set = 0;
+			break;
+		}
+#endif
 		parse_line(&l, strdup(line));
 		if (cur.n && strcmp(cur.lines[0].f[0], l.f[0]) != 0) CLOSE_BLOCK();
 		if (cur.n == cur.m) { cur.m = cur.m ? cur.m * 2 : 4; cur.lines = (line_t*)realloc(cur.lines, sizeof(line_t) * cur.m); }
@@ -364,6 +450,9 @@ int main(int argc, char **argv)
 	if (splitfn) fprintf(stderr, "samblaster: Output %llu split reads to %s\n", o.n_split / 2, splitfn);
 	fprintf(stderr, "samblaster: Marked %llu of %llu (%.2f%%) read ids as duplicates.\n", o.n_dup, o.n_ids, o.n_ids ? 100.0 * o.n_dup / o.n_ids : 0.0);
 	if (set) ssq_dupset_free(set);
+#ifdef SSQ_SB_DEVICE_TEXT
+	free(hdr);
+#endif
 	free(line); free(blocks); free(sigs); free(dups); free(meta);
 	return 0;
 }
