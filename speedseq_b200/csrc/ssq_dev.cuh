@@ -64,7 +64,8 @@ struct DevIndex {
 
 struct Counters { // device-measured work, feeds roofline.achieved (algorithmic bytes, SURVEY.md §8d)
 	unsigned long long occ_smem, occ_sa, sa_reads, sw_calls, sw_cells, sw_bytes, n_seeds, n_regs;
-	unsigned long long dbg[16]; // kernel-internal cycle counters (diagnostics); [8..11]: rank-block counter before/after the two backward-sweep launches
+	unsigned long long dbg[16]; // kernel-internal cycle counters (diagnostics); [8..11]: rank-block counter before/after the two backward-sweep launches;
+	                            // [12]: seeding queries answered from the k-mer table, [13]: seeding extensions through occ4_pair()
 };
 
 template <class U> struct IntvT { U x0, x1, x2; u32 qb, qe; }; // bi-interval + query span [qb,qe)
@@ -137,8 +138,8 @@ SSQ_HD void blk32_count(const Blk32 &b, U kk, U cnt[4])
 
 struct ScalarFm {
 	const DevIndex &ix;
-	unsigned long long n_blk;
-	SSQ_HD ScalarFm(const DevIndex &i) : ix(i), n_blk(0) {}
+	u32 n_blk, n_step, n_tab; // rank blocks (sectors) loaded; extensions through occ4_pair(); queries answered from the k-mer table
+	SSQ_HD ScalarFm(const DevIndex &i) : ix(i), n_blk(0), n_step(0), n_tab(0) {}
 	SSQ_HD void occ4(u64 k, u64 cnt[4])
 	{
 		if (k == (u64)-1) { cnt[0] = cnt[1] = cnt[2] = cnt[3] = 0; return; }
@@ -170,6 +171,25 @@ struct ScalarFm {
 		++n_blk;
 		blk32_count(b, kk, cnt);
 	}
+	// both ends of an extension: counts up to rows k0 and k1 (k0 <= k1: the row before an interval and its last row)
+	SSQ_HD void occ4_pair(u64 k0, u64 k1, u64 tk[4], u64 tl[4]) { ++n_step; occ4(k0, tk); occ4(k1, tl); }
+	// 32-bit rows: once a string is longer than ~16 bases its interval spans a few rows, and both ends often lie in the same 64-row
+	// block (36 % of the steps on the bench workload).  That block is then loaded once and both count vectors come from the same
+	// registers (one sector instead of two); otherwise both loads are issued before either block is used (one round trip either way).
+	SSQ_HD void occ4_pair(u32 k0, u32 k1, u32 tk[4], u32 tl[4])
+	{
+		++n_step;
+		const u32 p = (u32)ix.primary, kk1 = k1 - (k1 >= p);
+		const bool none0 = k0 == (u32)-1; // the interval starts at row 0: nothing before it (counted from k1's block, then cleared)
+		const u32 kk0 = none0 ? kk1 : k0 - (k0 >= p);
+		const Blk32 b0 = load_blk32(ix.bwt32 + ((size_t)(kk0 >> 6) << 3));
+		Blk32 b1 = b0;
+		if ((kk0 ^ kk1) >> 6) { b1 = load_blk32(ix.bwt32 + ((size_t)(kk1 >> 6) << 3)); ++n_blk; } // issued before either block is used
+		++n_blk;
+		blk32_count(b1, kk1, tl);
+		blk32_count(b0, kk0, tk);
+		if (none0) tk[0] = tk[1] = tk[2] = tk[3] = 0;
+	}
 	// ok[c] of a forward (is_back=0) or backward (is_back=1) extension of ik by every base c
 	SSQ_HD void extend(const Intv &ik, Intv ok[4], int is_back)
 	{
@@ -199,8 +219,7 @@ SSQ_HD void extend1(Fm &fm, const IntvT<U> &ik, int c, int is_back, IntvT<U> &ou
 	const DevIndex &ix = fm.ix;
 	U tk[4], tl[4];
 	const U kf = is_back ? ik.x0 : ik.x1, ko = is_back ? ik.x1 : ik.x0;
-	fm.occ4((U)(kf - 1), tk);
-	fm.occ4((U)(kf - 1 + ik.x2), tl);
+	fm.occ4_pair((U)(kf - 1), (U)(kf - 1 + ik.x2), tk, tl);
 	const U n0 = tl[0] - tk[0], n1 = tl[1] - tk[1], n2 = tl[2] - tk[2], n3 = tl[3] - tk[3];
 	const U nf = SSQ_SEL4((U)ix.L2[0] + 1 + tk[0], (U)ix.L2[1] + 1 + tk[1], (U)ix.L2[2] + 1 + tk[2], (U)ix.L2[3] + 1 + tk[3], c);
 	const U base = ko + (U)(kf <= (U)ix.primary && (U)(kf + ik.x2 - 1) >= (U)ix.primary);
@@ -222,6 +241,9 @@ SSQ_HD void set_intv(const DevIndex &ix, int c, IntvT<U> &ik)
 // sweeps.  The bi-interval of a string does not depend on how it was reached, so those queries can be answered — exactly — from a
 // table of the bi-intervals of all strings of length 1..K: entry (L, code) at kmer_off(L) + code, code = the L bases as a 2L-bit
 // number, first base in the top bits.  K = 10: 1.4 M entries x 16 B = 22 MB (L2-resident).  Indexes with < 2^32 rows only.
+// Built at index load for every bwt32 index (SSQ_KMER_K overrides K, 0 turns it off) and read by the forward walks (k_smem_fwd,
+// k_smem_p3).  K = 10 from an H100 sweep of K = 0, 8, 9, 10 on the bench workload (DESIGN.md §8); K = 11 (89 MB) is not L2-resident.
+#define SSQ_KMER_K_DEFAULT 10
 struct KmerEnt { u32 x0, x1, x2, pad; };
 SSQ_HD u32 kmer_off(int L) { return ((1u << (2 * L)) - 4u) / 3u; } // 4 + 16 + ... + 4^(L-1)
 SSQ_HD u32 kmer_entries(int K) { return kmer_off(K + 1); }

@@ -190,8 +190,8 @@ extern "C" int ssq_index_load(const char *prefix, int device, ssq_index_t **out)
 			idx->dev.sad_intv = d; idx->dev_bytes += nd * (small ? 4 : 8);
 		}
 	}
-	{ // k-mer jump-start table for the seeding kernels (SSQ_KMER_K=1..12; off by default until measured on the GPU)
-		const int K = getenv("SSQ_KMER_K") ? atoi(getenv("SSQ_KMER_K")) : 0;
+	{ // k-mer jump-start table for the seeding kernels: K = SSQ_KMER_K (1..12; 0 = no table), else SSQ_KMER_K_DEFAULT (see ssq_dev.cuh)
+		const int K = getenv("SSQ_KMER_K") ? atoi(getenv("SSQ_KMER_K")) : SSQ_KMER_K_DEFAULT;
 		if (K >= 1 && K <= 12 && idx->dev.bwt32) {
 			const u32 ne = kmer_entries(K);
 			void *dk = 0;

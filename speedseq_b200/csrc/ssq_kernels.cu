@@ -4,7 +4,8 @@
 //   seeding  a4  default: phase-split kernels — forward walks (k_smem_fwd<1|2>, lane = read), backward sweeps (k_smem_bwd, lane = call),
 //                pass-2 selection (k_smem_p2sel), greedy pass (k_smem_p3), one radix sort on (read, qb, qe) to publish the intervals.
 //                Indexes with >= 2^32 rows: the per-lane state machine k_smem_m<u64> + k_smem_p3 on the 64-byte on-disk rank blocks.
-//                Two back-to-back 128-bit loads per rank query of the re-blocked 32-byte sectors.  Bound: random sector reads (L2 / HBM).
+//                One sector (two back-to-back 128-bit loads) per extension whose interval ends share a 64-row block, two otherwise;
+//                the forward walks and the greedy pass take strings of <= K bases from the k-mer jump-start table.  Bound: random sector reads (L2 / HBM).
 //   k_sa     a5  thread per seed occurrence, LF walk to the load-time densified SA sample.  Same bound.
 //   k_chain / k_chain_coop  a6  per-lane ChainBuilder for reads with <= 16 seeds, warp per read (shared-memory chains, three
 //                capacity levels) above.
@@ -27,6 +28,19 @@
 #include "ssq_batch.h"
 
 #define FULL 0xffffffffu
+
+// a seeding kernel's rank-query counters: sectors loaded (counter 0), extensions through occ4_pair() and queries answered from the
+// k-mer table (diagnostic slots 13 and 12); the step counts are summed over the warp first
+__device__ __forceinline__ void fm_counters_flush(const ScalarFm &fm, Counters *cnt)
+{
+	const unsigned m = __activemask();
+	const u32 st = __reduce_add_sync(m, fm.n_step), tb = __reduce_add_sync(m, fm.n_tab);
+	if ((int)(threadIdx.x & 31) == __ffs(m) - 1) {
+		if (st) atomicAdd(&cnt->dbg[13], (unsigned long long)st);
+		if (tb) atomicAdd(&cnt->dbg[12], (unsigned long long)tb);
+	}
+	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+}
 
 // ------------------------------------------------------------------ warp-cooperative FM context ----
 struct WarpFm {
@@ -149,7 +163,7 @@ __global__ void __launch_bounds__(128) k_smem_t(DevIndex ix, ssq_opts_t opt, int
 		for (int i = 0; i < n; ++i) pool[base + i] = mem[i];
 		intv_off[r] = base; intv_cnt[r] = n; l_rep_out[r] = l_rep;
 	}
-	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+	fm_counters_flush(fm, cnt);
 }
 
 // state-machine variant (default): a lane owns one machine and keeps pulling reads from the work counter; the only step
@@ -225,7 +239,7 @@ __global__ void __launch_bounds__(256) k_smem_p3(DevIndex ix, ssq_opts_t opt, in
 		if (ready) {
 			IntvT<U> okc;
 			if (TAB) code = code << 2 | (u32)qi;
-			if (TAB && i + 1 - x <= ix.kmer_k) { const Intv32 t = kmer_lookup(ix, i + 1 - x, code); okc.x0 = (U)t.x0; okc.x1 = (U)t.x1; okc.x2 = (U)t.x2; okc.qb = okc.qe = 0; }
+			if (TAB && i + 1 - x <= ix.kmer_k) { const Intv32 t = kmer_lookup(ix, i + 1 - x, code); okc.x0 = (U)t.x0; okc.x1 = (U)t.x1; okc.x2 = (U)t.x2; okc.qb = okc.qe = 0; ++fm.n_tab; }
 			else extend1(fm, ik, 3 - qi, 0, okc);
 			if (okc.x2 < max_intv && i - x >= min_len) {
 				if (okc.x2 > 0 && n_out < stride) { Intv m = widen(okc); m.qb = (u32)x; m.qe = (u32)(i + 1); p3[(size_t)r * stride + n_out] = m; }
@@ -238,7 +252,8 @@ __global__ void __launch_bounds__(256) k_smem_p3(DevIndex ix, ssq_opts_t opt, in
 			}
 		}
 	}
-	if (fm.n_blk) { atomicAdd(&cnt->occ_smem, fm.n_blk); atomicAdd(&cnt->dbg[6], fm.n_blk); } // dbg[6]: this kernel's share of occ_smem
+	fm_counters_flush(fm, cnt);
+	if (fm.n_blk) atomicAdd(&cnt->dbg[6], fm.n_blk); // dbg[6]: this kernel's share of occ_smem
 }
 
 template <class U, int MINB, bool TAB>
@@ -306,12 +321,12 @@ __global__ void __launch_bounds__(128, MINB) k_smem_m(DevIndex ix, ssq_opts_t op
 		}
 		if (ready) { // the step all lanes that have a query take together
 			IntvT<U> okc;
-			if (!(TAB && m.table_hit(ix, okc))) extend1(fm, m.in, m.qc, m.is_back, okc);
+			if (TAB && m.table_hit(ix, okc)) ++fm.n_tab; else extend1(fm, m.in, m.qc, m.is_back, okc);
 			m.post(okc);
 			ready = false;
 		}
 	}
-	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+	fm_counters_flush(fm, cnt);
 }
 
 // ------------------------------------------------------- phase-split seeding (variant 3) ----
@@ -405,7 +420,7 @@ __global__ void __launch_bounds__(256) k_smem_fwd(DevIndex ix, ssq_opts_t opt, i
 		if (ready) {
 			Intv32 okc;
 			if (TAB) code = code << 2 | (u32)qi;
-			if (TAB && i + 1 - x <= ix.kmer_k) okc = kmer_lookup(ix, i + 1 - x, code); else extend1(fm, ik, 3 - qi, 0, okc);
+			if (TAB && i + 1 - x <= ix.kmer_k) { okc = kmer_lookup(ix, i + 1 - x, code); ++fm.n_tab; } else extend1(fm, ik, 3 - qi, 0, okc);
 			bool end = false;
 			if (okc.x2 != ik.x2) { push(); end = okc.x2 < min_intv; }
 			if (!end) {
@@ -416,10 +431,11 @@ __global__ void __launch_bounds__(256) k_smem_fwd(DevIndex ix, ssq_opts_t opt, i
 			if (end) flush();
 		}
 	}
-	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+	fm_counters_flush(fm, cnt);
 }
 
-// backward sweeps of the calls [lo, hi): lane = call
+// backward sweeps of the calls [lo, hi): lane = call.  No k-mer table here: a warp whose lanes split between table entries (L2) and
+// rank blocks (HBM) waits for both in turn, and on the H100 that made the two launches 2.6 ms slower per 1 M reads at K = 10 (DESIGN §8)
 template <int MINB>
 __global__ void __launch_bounds__(128, MINB) k_smem_bwd(DevIndex ix, ssq_opts_t opt, const uint8_t *__restrict__ seq, const u64 *__restrict__ read_off, int lcap, int list_cap,
                                                         Intv *scratch, int scratch_cap, const SeedCall *__restrict__ calls, const FwdEntry *__restrict__ fl, int second,
@@ -465,7 +481,7 @@ __global__ void __launch_bounds__(128, MINB) k_smem_bwd(DevIndex ix, ssq_opts_t 
 			ready = m.advance(ix);
 		}
 	}
-	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+	fm_counters_flush(fm, cnt);
 }
 
 // the same kernel with the lean per-lane state (BwdCallT): fewer registers -> more blocks per SM, fewer instructions per step
@@ -511,12 +527,12 @@ __global__ void __launch_bounds__(128, MINB) k_smem_bwd2(DevIndex ix, ssq_opts_t
 		if (__ballot_sync(FULL, alive) == 0) break;
 		if (ready) {
 			Intv32 okc;
-			if (!(TAB && m.table_hit(ix, okc))) extend1(fm, m.in, m.c, 1, okc);
+			if (TAB && m.table_hit(ix, okc)) ++fm.n_tab; else extend1(fm, m.in, m.c, 1, okc);
 			m.post(okc);
 			ready = m.advance();
 		}
 	}
-	if (fm.n_blk) atomicAdd(&cnt->occ_smem, fm.n_blk);
+	fm_counters_flush(fm, cnt);
 }
 
 // range bookkeeping between the kernels; the counters keep counting when a pool is full, the ranges the next kernels walk must not
@@ -1470,10 +1486,12 @@ static int run_smem_split(ssq_batch *b)
 	const bool lean = b->smem_variant == 4;
 	const int lean_blocks = getenv("SSQ_SMEM_BLOCKS") ? atoi(getenv("SSQ_SMEM_BLOCKS")) : 8;
 	typedef void (*bwd_kernel_t)(DevIndex, ssq_opts_t, const uint8_t*, const u64*, int, int, Intv*, int, const SeedCall*, const FwdEntry*, int, Intv*, u32*, u64, Split*, Counters*);
-	const int bwd_blocks = getenv("SSQ_SMEM_BWD_BLOCKS") ? atoi(getenv("SSQ_SMEM_BWD_BLOCKS")) : 6; // resident blocks per SM the backward kernel is compiled for (register budget)
-	const bwd_kernel_t kb = bwd_blocks >= 8 ? k_smem_bwd<8> : bwd_blocks == 7 ? k_smem_bwd<7> : k_smem_bwd<6>;
+	// resident blocks per SM the backward kernel is compiled for (register budget): 5 leaves the one-sector step both loads in flight
+	// without spilling (94 registers); at 6 (80 registers) it spills and the two launches took 44 ms instead of 36 per 1 M reads
+	const int bwd_blocks = getenv("SSQ_SMEM_BWD_BLOCKS") ? atoi(getenv("SSQ_SMEM_BWD_BLOCKS")) : 5;
+	const bwd_kernel_t kb = bwd_blocks >= 8 ? k_smem_bwd<8> : bwd_blocks == 7 ? k_smem_bwd<7> : bwd_blocks == 6 ? k_smem_bwd<6> : k_smem_bwd<5>;
 	CK(cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)bthreads * 2 * (list_cap > 0 ? list_cap : 1) * sizeof(uint4))));
-	const bool tab = b->idx->dev.kmer_k > 0; // k-mer jump-start table loaded (SSQ_KMER_K): forward walks, the greedy pass and the lean backward kernel use it
+	const bool tab = b->idx->dev.kmer_k > 0; // k-mer jump-start table loaded (by default for bwt32 indexes): forward walks, the greedy pass and the lean backward kernel use it
 	typedef void (*fwd_kernel_t)(DevIndex, ssq_opts_t, int, const uint8_t*, const u64*, int, FwdEntry*, SeedCall*, u64, FwdEntry*, u64, Split*, Counters*);
 	typedef void (*bwd2_kernel_t)(DevIndex, ssq_opts_t, const uint8_t*, int, int, Intv*, int, const SeedCall*, const FwdEntry*, int, Intv*, u32*, u64, Split*, Counters*);
 	const fwd_kernel_t kf1 = tab ? k_smem_fwd<1, true> : k_smem_fwd<1, false>, kf2 = tab ? k_smem_fwd<2, true> : k_smem_fwd<2, false>;
@@ -1893,6 +1911,8 @@ extern "C" uint64_t ssq_batch_counter(const ssq_batch_t *b_, int what)
 	case 9: return b->n_intv; case 10: return b->n_tasks; case 11: return (uint64_t)b->ext_rounds;
 	case 12: case 13: case 14: case 15: case 16: return b->h_cnt.dbg[what - 12];
 	case 23: return b->h_cnt.dbg[6]; // rank blocks dereferenced by k_smem_p3 (part of counter 0)
+	case 27: return b->h_cnt.dbg[12]; // seeding rank queries answered from the k-mer jump-start table
+	case 28: return b->h_cnt.dbg[13]; // seeding rank queries answered from rank blocks: each loads one sector (both interval ends in one block) or two; counter 0 = sectors
 	case 25: return (b->h_cnt.dbg[9] - b->h_cnt.dbg[8]) + (b->h_cnt.dbg[11] - b->h_cnt.dbg[10]); // rank blocks dereferenced by the two backward-sweep launches (split seeding)
 	case 26: { float m1 = 0.f, m2 = 0.f; if (cudaEventElapsedTime(&m1, b->evb[0], b->evb[1]) != cudaSuccess || cudaEventElapsedTime(&m2, b->evb[2], b->evb[3]) != cudaSuccess) { cudaGetLastError(); return 0; } return (uint64_t)((m1 + m2) * 1000.f); } // their duration, microseconds
 	case 24: { float ms = 0.f; if (cudaEventElapsedTime(&ms, b->evs[0], b->evs[1]) != cudaSuccess) { cudaGetLastError(); return 0; } return (uint64_t)(ms * 1000.f); } // k_smem_m alone, microseconds
