@@ -338,6 +338,13 @@ int ssq_gunzip_inflate(ssq_gunzip_t *g, const void *in, size_t n, int final, siz
 /* a whole stream, device buffers, on the object's stream (returns after it is done); SSQ_ECAP with *out_len = the text's size
  * when it does not fit.  Independent of the streaming state. */
 int ssq_gunzip_inflate_dev(ssq_gunzip_t *g, const void *d_in, size_t n, void *d_out, size_t out_cap, size_t *out_len);
+/* BGZF, member-parallel (what BAI virtual offsets are made of): the members are found by walking the BSIZE chain (the BC extra
+ * subfield) from byte 0, each is decoded as its own chunk and checked against its CRC-32 and ISIZE.  Device buffers, on the object's
+ * stream.  members: host array of 2 * members_cap values, (compressed offset, text offset) of member k at [2k, 2k + 1].
+ * SSQ_EDATA: a member without BSIZE, a chain that does not land on a member header or does not end exactly at n, a truncated or
+ * corrupt member, ISIZE over 64 KB.  SSQ_ECAP (with *out_len and *n_members set): the text or the table does not fit.  Leaves
+ * ssq_gunzip_stats alone. */
+int ssq_gunzip_inflate_bgzf_dev(ssq_gunzip_t *g, const void *d_in, size_t n, void *d_out, size_t out_cap, size_t *out_len, uint64_t *members, size_t members_cap, size_t *n_members);
 /* since create: chunks decoded, chunks started at a searched sync point, chunks decoded again after a broken link, windows */
 int ssq_gunzip_stats(const ssq_gunzip_t *g, int64_t out[4]);
 void *ssq_gunzip_stream(ssq_gunzip_t *g);           /* cudaStream_t of the object, for event timing */
@@ -386,6 +393,25 @@ int ssq_sam2bam_create(int device, const char *header, size_t header_len, ssq_sa
 int ssq_sam2bam_run(ssq_sam2bam_t *t, const char *text, size_t len, int final, size_t *used, const void **run, size_t *run_len, uint64_t *n_records);
 void *ssq_sam2bam_stream(ssq_sam2bam_t *t);         /* cudaStream_t of the object, for event timing */
 void ssq_sam2bam_free(ssq_sam2bam_t *t);
+/* The BAI index of a coordinate-sorted BAM file on the device (csrc/ssq_bai.cu): what `sambamba index in.bam` (0.5.9) writes to
+ * in.bam.bai, byte for byte — the call speedseq makes on each BAM of `align` and `realign` (speedseq:486-494, :1983-1985,
+ * :2016-2023), and what sambamba's `sort -o` writes next to its output.  The rules and what is refused are at the head of
+ * csrc/ssq_bai.cuh; in short, SSQ_EDATA for input that is not BGZF or does not inflate, SSQ_EFORMAT (with the record in
+ * ssq_last_error()) for a text that is not a BAM file, records out of coordinate order, a refID outside the header, a record with
+ * a reference and no position, a record that reaches past 2^29, a record without a reference before one with one, and an empty
+ * BGZF member before the last.  seg_bytes: text per record walker (0 = 64 KB).  One host thread at a time per object; without a
+ * usable GPU create returns SSQ_ENOGPU. */
+typedef struct ssq_bai ssq_bai_t;
+int ssq_bai_create(int device, size_t seg_bytes, ssq_bai_t **out);
+/* bam[0, len): the whole BAM file (host memory; staged through pinned memory).  *bai_out: the index file's bytes, free with
+ * ssq_free. */
+int ssq_bai_build(ssq_bai_t *b, const void *bam, size_t len, void **bai_out, size_t *bai_len);
+/* time of the last build in ms between CUDA events on the object's stream: 0 the input's staging through pinned memory, its copy
+ * in and the BGZF inflation (host work between the member rounds included), 1 record walk and checks, 2 index assembly and the
+ * copy back (the host's link checks and waits included in each) */
+int ssq_bai_times(const ssq_bai_t *b, float ms[3]);
+void *ssq_bai_stream(ssq_bai_t *b);                 /* cudaStream_t of the object, for event timing */
+void ssq_bai_free(ssq_bai_t *b);
 /* the sorted runs of consecutive batches -> one sorted record stream (stable: equal keys keep batch order); free with ssq_free */
 int ssq_bam_merge_runs(int n_runs, const void *const *runs, const size_t *lens, void **out, size_t *out_len);
 

@@ -369,3 +369,53 @@ class SSQ:
 
     def sam2bam_free(self, t):
         self.lib.ssq_sam2bam_free(t)
+
+    # ---- BAI index of a sorted BAM on the device (ssq_bai_*, ssq_gunzip_inflate_bgzf_dev) ----
+    def gunzip_inflate_bgzf_dev(self, g, d_in, n, d_out, out_cap, members_cap):
+        """device pointers (ints) -> (rc, out_len, [(compressed offset, text offset)] of the members); rc is 0, SSQ_ECAP (-5) or
+        SSQ_EDATA (-9)"""
+        ln, nm = C.c_size_t(0), C.c_size_t(0)
+        mt = np.zeros(max(2 * members_cap, 2), np.uint64)
+        rc = self.lib.ssq_gunzip_inflate_bgzf_dev(g, C.c_void_p(d_in), C.c_size_t(n), C.c_void_p(d_out), C.c_size_t(out_cap), C.byref(ln), _ptr(mt),
+                                                  C.c_size_t(members_cap), C.byref(nm))
+        if rc not in (0, -5, -9):
+            self.ck(rc, "ssq_gunzip_inflate_bgzf_dev")
+        return rc, int(ln.value), [(int(mt[2 * k]), int(mt[2 * k + 1])) for k in range(nm.value)] if rc == 0 else []
+
+    def bai_create(self, device=0, seg_bytes=0):
+        L = self.lib
+        L.ssq_bai_create.argtypes = [C.c_int, C.c_size_t, C.c_void_p]
+        L.ssq_bai_build.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        L.ssq_bai_times.argtypes = [C.c_void_p, C.c_void_p]
+        L.ssq_bai_stream.restype = C.c_void_p
+        L.ssq_bai_stream.argtypes = [C.c_void_p]
+        L.ssq_bai_free.argtypes = [C.c_void_p]
+        L.ssq_free.argtypes = [C.c_void_p]
+        h = C.c_void_p()
+        self.ck(L.ssq_bai_create(C.c_int(device), C.c_size_t(seg_bytes), C.byref(h)), "ssq_bai_create")
+        return h
+
+    def bai_build(self, b, bam):
+        """the index of a whole BAM file (bytes) -> (rc, index bytes); rc is 0, SSQ_EDATA (-9) or SSQ_EFORMAT (-8), whose message
+        ssq_last_error() holds"""
+        out, n = C.c_void_p(), C.c_size_t(0)
+        rc = self.lib.ssq_bai_build(b, bam, C.c_size_t(len(bam)), C.byref(out), C.byref(n))
+        if rc not in (0, -8, -9):
+            self.ck(rc, "ssq_bai_build")
+        if rc:
+            return rc, b""
+        data = C.string_at(out, n.value)
+        self.lib.ssq_free(out)
+        return 0, data
+
+    def bai_times(self, b):
+        """device ms of the last build: (BGZF inflation, record walk and checks, index assembly)"""
+        ms = (C.c_float * 3)()
+        self.ck(self.lib.ssq_bai_times(b, ms), "ssq_bai_times")
+        return tuple(ms)
+
+    def bai_stream(self, b):
+        return self.lib.ssq_bai_stream(b)
+
+    def bai_free(self, b):
+        self.lib.ssq_bai_free(b)

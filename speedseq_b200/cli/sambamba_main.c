@@ -14,7 +14,12 @@
  * converted and sorted by ssq_sam2bam_run.  Its output is only meaningful to this shim's `sort` — true of every call site in
  * speedseq, which the program cannot see, hence the opt-in.  A refused line, a CUDA error or no GPU: one stderr line, an abort
  * frame (ssq_fuse.h), a non-zero exit; `sort` then exits non-zero without creating -o.
- * Everything else — other subcommands (index, merge, ...), and view / sort whose stdin is ordinary SAM / BAM (without
+ * After the merge, `sort -o out.bam` writes out.bam.bai, as sambamba 0.5.9's sort does, with the builder of `index`.
+ *   index: `index [-t N] [-p] in.bam [out.bai]` (speedseq:486-494, :1983-1985, :2016-2023) runs on the device (ssq_bai_build,
+ *          byte-identical to sambamba's index; -t and -p change nothing).  -c / --check-bins, -C / CRAM, other options, input that
+ *          is not BGZF, input the device refuses (its rules: csrc/ssq_bai.cuh) and no usable GPU go to the real sambamba after one
+ *          stderr line naming the reason; after `sort`, such a file is indexed by the real sambamba's `index`.
+ * Everything else — other subcommands (merge, ...), and view / sort whose stdin is ordinary SAM / BAM (without
  * SSQ_SAM2BAM_GPU, the splitter and discordant streams, speedseq:444-448) — goes to the real sambamba named by SSQ_SAMBAMBA_REAL
  * (or `sambamba.real` next to this executable) with the bytes already read handed on, so one SAMBAMBA= line serves the whole
  * script. */
@@ -394,6 +399,85 @@ static int view_sam2bam(head_t *h)
 	return 0;
 }
 
+/* ---- `index` on the device: the whole file is read, indexed by ssq_bai_build and the index written next to it ---- */
+/* 0: written; 1: the device path cannot take it (*why says why; nothing written); 2: the input cannot be read or the index written */
+static int bai_write(const char *in, const char *out, char *why, size_t why_len)
+{
+	FILE *fp = fopen(in, "rb");
+	uint8_t *buf = 0;
+	size_t n = 0, cap = 0, k;
+	void *bai = 0; size_t bai_len = 0;
+	ssq_bai_t *b = 0;
+	const char *dv = getenv("SSQ_DEVICE");
+	int rc;
+	if (!fp) { snprintf(why, why_len, "cannot open %s: %s", in, strerror(errno)); return 1; } /* the real sambamba reports it in its own words */
+	for (;;) {
+		if (n == cap) { cap = cap ? cap * 2 : 1 << 24; buf = (uint8_t*)realloc(buf, cap); if (!buf) { fprintf(stderr, "sambamba (GPU shim): out of memory\n"); fclose(fp); return 2; } }
+		k = fread(buf + n, 1, cap - n, fp);
+		if (!k) break;
+		n += k;
+	}
+	if (ferror(fp)) { fprintf(stderr, "sambamba (GPU shim): cannot read %s: %s\n", in, strerror(errno)); fclose(fp); free(buf); return 2; }
+	fclose(fp);
+	if (n < 18 || buf[0] != 0x1f || buf[1] != 0x8b || buf[2] != 8 || !(buf[3] & 4)) { snprintf(why, why_len, "%s is not BGZF", in); free(buf); return 1; }
+	if ((rc = ssq_bai_create(dv && dv[0] ? atoi(dv) : 0, 0, &b))) { snprintf(why, why_len, "no usable GPU: %s", ssq_last_error()); free(buf); return 1; }
+	rc = ssq_bai_build(b, buf, n, &bai, &bai_len);
+	free(buf);
+	if (rc) { snprintf(why, why_len, "the device does not index %s: %s", in, ssq_last_error()); ssq_bai_free(b); return 1; }
+	ssq_bai_free(b);
+	if (!(fp = fopen(out, "wb"))) { fprintf(stderr, "sambamba (GPU shim): cannot create %s: %s\n", out, strerror(errno)); ssq_free(bai); return 2; }
+	if (fwrite(bai, 1, bai_len, fp) != bai_len || fclose(fp)) { fprintf(stderr, "sambamba (GPU shim): cannot write %s\n", out); ssq_free(bai); return 2; }
+	ssq_free(bai);
+	return 0;
+}
+static int index_main(int argc, char **argv)
+{
+	const char *in = 0, *out = 0;
+	char why[1200], def[4096];
+	int i, rc;
+	for (i = 2; i < argc; ++i) {
+		if ((!strcmp(argv[i], "-t") || !strcmp(argv[i], "--nthreads")) && i + 1 < argc) ++i; /* threads and progress change nothing on the device */
+		else if (!strncmp(argv[i], "--nthreads=", 11) || !strncmp(argv[i], "-t", 2) || !strcmp(argv[i], "-p") || !strcmp(argv[i], "--show-progress")) {}
+		else if (!strcmp(argv[i], "-c") || !strcmp(argv[i], "--check-bins")) { fprintf(stderr, "sambamba (GPU shim): index -c (bin check) is not on the GPU; running the real sambamba\n"); exec_real(argv, "`index -c`"); }
+		else if (!strcmp(argv[i], "-C") || !strcmp(argv[i], "--cram-input")) { fprintf(stderr, "sambamba (GPU shim): index of CRAM is not on the GPU; running the real sambamba\n"); exec_real(argv, "`index -C`"); }
+		else if (argv[i][0] == '-' && argv[i][1]) { fprintf(stderr, "sambamba (GPU shim): index option %s is not on the GPU; running the real sambamba\n", argv[i]); exec_real(argv, "this `index` option"); }
+		else if (!in) in = argv[i];
+		else if (!out) out = argv[i];
+		else exec_real(argv, "`index` with more than two files");
+	}
+	if (!in) exec_real(argv, "`index` without input");
+	if (!out) { snprintf(def, sizeof def, "%s.bai", in); out = def; }
+	rc = bai_write(in, out, why, sizeof why);
+	if (rc == 1) { fprintf(stderr, "sambamba (GPU shim): %s; running the real sambamba\n", why); exec_real(argv, "this `index`"); }
+	return rc;
+}
+/* after `sort -o`: out.bam.bai, as sambamba's sort writes it — the same builder as `index`, or the real sambamba's index when the
+ * device cannot take the file.  When neither can write it (no real sambamba, or it fails), one stderr line says so and the sort
+ * still succeeds: the sorted file is complete and correct, and every caller in speedseq runs `$SAMBAMBA index` on it next
+ * (speedseq:486-494, :1983-1985, :2016-2023), which then builds the index or fails with its own message.  Failing the sort instead
+ * would make the script discard a good BAM over its side file. */
+static int sort_index(const char *out_fn)
+{
+	char bai_fn[4096], why[1200];
+	int rc, st = 0;
+	pid_t pid;
+	snprintf(bai_fn, sizeof bai_fn, "%s.bai", out_fn);
+	rc = bai_write(out_fn, bai_fn, why, sizeof why);
+	if (rc != 1) return rc ? 1 : 0;
+	{
+		const char *r = real_path();
+		char *av[4];
+		if (!r) { fprintf(stderr, "sambamba (GPU shim): %s; %s is not written (no real sambamba to index with)\n", why, bai_fn); return 0; }
+		fprintf(stderr, "sambamba (GPU shim): %s; indexing %s with the real sambamba\n", why, out_fn);
+		av[0] = (char*)r; av[1] = (char*)"index"; av[2] = (char*)out_fn; av[3] = 0;
+		if ((pid = fork()) < 0) { perror("fork"); return 1; }
+		if (pid == 0) { execv(r, av); _exit(127); }
+		while (waitpid(pid, &st, 0) < 0 && errno == EINTR) {}
+		if (!WIFEXITED(st) || WEXITSTATUS(st)) fprintf(stderr, "sambamba (GPU shim): the real sambamba did not index %s\n", out_fn);
+		return 0;
+	}
+}
+
 int main(int argc, char **argv)
 {
 	head_t h;
@@ -446,8 +530,10 @@ int main(int argc, char **argv)
 		if (!sniff_runs(&h, &body)) return feed_real(argv, h.p, h.n, "`sort` of ordinary BAM");
 		if (by_name || !out_fn) { fprintf(stderr, "sambamba (GPU shim): the run stream can only be coordinate-sorted into a file (-o)\n"); return 1; }
 		if (getenv("SSQ_SORT_SPILL_BYTES")) mem_limit = 2 * (size_t)atoll(getenv("SSQ_SORT_SPILL_BYTES")); /* tests: force the spill path on small inputs */
-		return sort_runs(&h, body, out_fn, threads, level, mem_limit / 2, tmpdir);
+		if (sort_runs(&h, body, out_fn, threads, level, mem_limit / 2, tmpdir)) return 1;
+		return sort_index(out_fn);
 	}
+	if (!strcmp(argv[1], "index")) return index_main(argc, argv);
 	exec_real(argv, "this subcommand");
 	return 1;
 }

@@ -3,7 +3,9 @@
 // CTA over the chunk tails in order, then a block per chunk; CRC: a thread per piece), driven window by window by gz_window.
 // Grids are sized from the SM count.  Device memory per object is fixed at create: GZ_MAXCH slots of GZ_SLOT 16-bit symbols (1 GB),
 // the window's text behind 32 KB of context (512 MB) and the window's compressed input (GZ_MAXCH chunks + 1 MB).
-// C-ABI: ssq_gunzip_create / ssq_gunzip_inflate / ssq_gunzip_inflate_dev / ssq_gunzip_stats (include/ssq.h).
+// BGZF (ssq_gunzip_inflate_bgzf_dev): one thread walks the BSIZE chain, then the decode kernel runs one member per thread (a block of one thread), GZ_MAXCH
+// members at a time, each writing its text at its final place, and the CRC kernel checks them.  ssq_gunzip_stats counts neither.
+// C-ABI: ssq_gunzip_create / ssq_gunzip_inflate / ssq_gunzip_inflate_dev / ssq_gunzip_inflate_bgzf_dev / ssq_gunzip_stats (include/ssq.h).
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
@@ -58,6 +60,36 @@ __global__ void __launch_bounds__(256) k_gz_crc(const uint8_t *wout, const bz_u6
 	tab[threadIdx.x] = bz_crc_entry(threadIdx.x);
 	__syncthreads();
 	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = gz_crc_piece(tab, wout + GZ_CTX + off[i], len[i]);
+}
+
+
+// ---- BGZF: chunk i is member i (gz_bgzf_members) ----
+__global__ void k_gz_bgzf_chain(const uint8_t *in, bz_u64 n, GzMember *m, bz_u64 cap, bz_u64 *res)
+{
+	if (threadIdx.x || blockIdx.x) return;
+	bz_u64 nm = 0, at = 0;
+	const int r = gz_bgzf_chain(in, n, m, cap, &nm, &at);
+	res[0] = (bz_u64)r; res[1] = nm; res[2] = at; res[3] = nm ? m[nm - 1].toff + m[nm - 1].isize : 0;
+}
+// one thread per block, one member per thread: the Huffman tables of its block in shared memory
+__global__ void __launch_bounds__(1) k_gz_bgzf_decode(const uint8_t *in, const GzMember *m, int k, GzChunk *ch, GzEvent *ev, uint16_t *slots)
+{
+	__shared__ GzTab T;
+	for (int i = blockIdx.x; i < k; i += gridDim.x) {
+		GzIn I; I.p = in + m[i].coff; I.n = m[i].csize; I.final = 1;
+		gz_decode(I, T, ch[i], slots + (bz_u64)i * GZ_SLOT, ev + (bz_u64)i * GZ_EVCAP);
+	}
+}
+__global__ void __launch_bounds__(256) k_gz_bgzf_emit(const uint16_t *slots, const GzMember *m, int k, uint8_t *out)
+{
+	for (int i = blockIdx.x; i < k; i += gridDim.x) gz_bgzf_emit(slots + (bz_u64)i * GZ_SLOT, m[i].isize, out + m[i].toff, threadIdx.x, blockDim.x);
+}
+__global__ void __launch_bounds__(256) k_gz_bgzf_crc(const uint8_t *out, const bz_u64 *off, const u32 *len, int n, u32 *res)
+{
+	__shared__ u32 tab[256];
+	tab[threadIdx.x] = bz_crc_entry(threadIdx.x);
+	__syncthreads();
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) res[i] = gz_crc_piece(tab, out + off[i], len[i]);
 }
 
 struct DevBackend : GzBackend {
@@ -129,6 +161,7 @@ struct ssq_gunzip {
 	size_t pend_cap, pend_len, pend_at;
 	GzState S;                        // the stream of ssq_gunzip_inflate
 	bz_u64 in_total;                     // compressed bytes of that stream already dropped
+	DBuf d_mt, d_res;                 // BGZF: the member table, the chain walk's result
 	std::vector<GzChunk> ch;
 	std::vector<GzEvent> ev;
 	int64_t stats[4];
@@ -210,6 +243,80 @@ extern "C" int ssq_gunzip_inflate_dev(ssq_gunzip_t *g, const void *d_in, size_t 
 	CK(cudaStreamSynchronize(g->be.st));
 	*out_len = S.total;
 	if (!fits) { ssq_set_error("ssq_gunzip_inflate_dev: %llu bytes of output, room for %zu", (unsigned long long)S.total, out_cap); return SSQ_ECAP; }
+	return SSQ_OK;
+}
+
+
+// the member-parallel path over the device's buffers of one ssq_gunzip object
+struct DevBgzf : GzBgzfBackend {
+	DevBackend *be; const uint8_t *in; uint8_t *out; const GzMember *h0, *d0;
+	int decode(const GzMember *m, int k, GzChunk *ch, GzEvent *ev) override
+	{
+		cudaStream_t st = be->st;
+		CK(cudaMemcpyAsync(be->d_ch.p, ch, (size_t)k * sizeof(GzChunk), cudaMemcpyHostToDevice, st));
+		k_gz_bgzf_decode<<<k < be->sms * 16 ? k : be->sms * 16, 1, 0, st>>>(in, d0 + (m - h0), k, be->d_ch.as<GzChunk>(), be->d_ev.as<GzEvent>(), be->d_slots.as<uint16_t>());
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(ch, be->d_ch.p, (size_t)k * sizeof(GzChunk), cudaMemcpyDeviceToHost, st));
+		CK(cudaMemcpyAsync(ev, be->d_ev.p, (size_t)k * GZ_EVCAP * sizeof(GzEvent), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		return 0;
+	}
+	int emit(const GzMember *m, int k) override
+	{
+		k_gz_bgzf_emit<<<k < be->sms * 8 ? k : be->sms * 8, 256, 0, be->st>>>(be->d_slots.as<uint16_t>(), d0 + (m - h0), k, out);
+		CK(cudaGetLastError());
+		return 0;
+	}
+	int crc(const std::vector<bz_u64> &off, const std::vector<u32> &len, std::vector<u32> &res) override
+	{
+		const int n = (int)off.size();
+		res.resize(n);
+		if (!n) return 0;
+		int rc;
+		if ((rc = be->d_poff.need((size_t)n * 8)) || (rc = be->d_plen.need((size_t)n * 4)) || (rc = be->d_pcrc.need((size_t)n * 4))) return rc;
+		CK(cudaMemcpyAsync(be->d_poff.p, off.data(), (size_t)n * 8, cudaMemcpyHostToDevice, be->st));
+		CK(cudaMemcpyAsync(be->d_plen.p, len.data(), (size_t)n * 4, cudaMemcpyHostToDevice, be->st));
+		const int blocks = (n + 255) / 256;
+		k_gz_bgzf_crc<<<blocks < be->sms * 8 ? blocks : be->sms * 8, 256, 0, be->st>>>(out, be->d_poff.as<bz_u64>(), be->d_plen.as<u32>(), n, be->d_pcrc.as<u32>());
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(res.data(), be->d_pcrc.p, (size_t)n * 4, cudaMemcpyDeviceToHost, be->st));
+		CK(cudaStreamSynchronize(be->st));
+		return 0;
+	}
+};
+
+extern "C" int ssq_gunzip_inflate_bgzf_dev(ssq_gunzip_t *g, const void *d_in, size_t n, void *d_out, size_t out_cap, size_t *out_len, uint64_t *members, size_t members_cap, size_t *n_members)
+{
+	if (!g || (!d_in && n) || (!d_out && out_cap) || !out_len || (!members && members_cap) || !n_members) { ssq_set_error("ssq_gunzip_inflate_bgzf_dev: invalid arguments"); return SSQ_EINVAL; }
+	*out_len = 0; *n_members = 0;
+	int rc = ssq_use_device(g->device);
+	if (rc) return rc;
+	// the member table: room for members of 8 KB or more (BGZF writers fill members to about 64 KB of text), walked again with
+	// room for the smallest possible members (28 bytes: header with BC, an empty deflate block, trailer) when that is short
+	cudaStream_t st = g->be.st;
+	bz_u64 res[4];
+	for (bz_u64 cap = n / 8192 + 64;; cap = n / 28 + 1) {
+		if ((rc = g->d_mt.need(cap * sizeof(GzMember))) || (rc = g->d_res.need(4 * 8))) return rc;
+		k_gz_bgzf_chain<<<1, 1, 0, st>>>((const uint8_t*)d_in, n, g->d_mt.as<GzMember>(), cap, g->d_res.as<bz_u64>());
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(res, g->d_res.p, sizeof res, cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		if (res[0] != GZ_B_CAP || cap == n / 28 + 1) break;
+	}
+	if (res[0]) { ssq_set_error("ssq_gunzip_inflate_bgzf_dev: not BGZF: %s at compressed byte %llu", gz_bgzf_why((int)res[0]), (unsigned long long)res[2]); return SSQ_EDATA; }
+	*out_len = res[3]; *n_members = res[1];
+	if (res[3] > out_cap || res[1] > members_cap) { ssq_set_error("ssq_gunzip_inflate_bgzf_dev: %llu bytes of text in %llu members, room for %zu and %zu", (unsigned long long)res[3], (unsigned long long)res[1], out_cap, members_cap); return SSQ_ECAP; }
+	std::vector<GzMember> m(res[1]);
+	if (res[1]) CK(cudaMemcpyAsync(m.data(), g->d_mt.p, res[1] * sizeof(GzMember), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	DevBgzf B; B.be = &g->be; B.in = (const uint8_t*)d_in; B.out = (uint8_t*)d_out; B.h0 = m.data(); B.d0 = g->d_mt.as<GzMember>();
+	bz_u64 at = 0;
+	if ((rc = gz_bgzf_members(B, m, &at))) {
+		if (rc == SSQ_EDATA) ssq_set_error("ssq_gunzip_inflate_bgzf_dev: corrupt BGZF member at compressed byte %llu (its deflate data, CRC-32 or ISIZE)", (unsigned long long)at);
+		return rc;
+	}
+	CK(cudaStreamSynchronize(st));
+	for (size_t k = 0; k < m.size(); ++k) { members[2 * k] = m[k].coff; members[2 * k + 1] = m[k].toff; }
 	return SSQ_OK;
 }
 

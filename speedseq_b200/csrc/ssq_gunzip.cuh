@@ -482,6 +482,98 @@ static inline int gz_window(GzBackend &be, GzState &S, const GzIn &I, bz_u64 chu
 static inline bz_u64 gz_consumed(const GzPos &p) { return (p.mode == GZ_M_IN ? p.hdr : p.bit) >> 3; }
 static inline void gz_rebase(GzPos &p, bz_u64 bytes) { p.bit -= bytes * 8; p.hdr -= bytes * 8; }
 
+// =============================================================== BGZF: chunk i is member i ====
+// A BGZF file is a chain of gzip members, each with a BC extra subfield (SLEN 2) holding BSIZE, the member's length - 1.  Walking
+// that chain gives every member's compressed offset; each member is an independent deflate stream of at most 64 KB of text, so
+// the chunk decode above runs on member i from its header (GZ_M_FIRST) to the end of the input it is given (the member): no sync
+// search, no placeholders, no link repair.  Member text offsets come from the ISIZE fields, so every member writes its text at
+// its final place; the CRC phase checks each member against its trailer.
+struct GzMember { bz_u64 coff, toff; u32 csize, isize; };
+enum { GZ_B_OK = 0, GZ_B_NOHDR = 1, GZ_B_NOBSIZE = 2, GZ_B_TRUNC = 3, GZ_B_BIG = 4, GZ_B_CAP = 5 };
+#define GZ_BGZF_MAX_ISIZE 65536u
+
+// the member at byte c: its length and ISIZE, or GZ_B_*
+SSQ_HD int gz_bgzf_member(const uint8_t *p, bz_u64 n, bz_u64 c, u32 *csize, u32 *isize)
+{
+	if (c + 12 > n) return GZ_B_TRUNC;
+	if (p[c] != 0x1f || p[c + 1] != 0x8b || p[c + 2] != 8) return GZ_B_NOHDR;
+	if (!(p[c + 3] & 4)) return GZ_B_NOBSIZE;
+	const u32 xlen = p[c + 10] | p[c + 11] << 8;
+	if (c + 12 + xlen > n) return GZ_B_TRUNC;
+	u32 bsize = 0; bool have = false;
+	for (u32 x = 0; x + 4 <= xlen;) {
+		const bz_u64 f = c + 12 + x;
+		const u32 slen = p[f + 2] | p[f + 3] << 8;
+		if (p[f] == 'B' && p[f + 1] == 'C' && slen == 2 && x + 6 <= xlen) { bsize = p[f + 4] | p[f + 5] << 8; have = true; break; }
+		x += 4 + slen;
+	}
+	if (!have) return GZ_B_NOBSIZE;
+	const bz_u64 len = (bz_u64)bsize + 1;
+	if (len < 12 + xlen + 8) return GZ_B_NOBSIZE; // BSIZE inside its own header: the chain cannot land on a member
+	if (c + len > n) return GZ_B_TRUNC;
+	*csize = (u32)len;
+	*isize = p[c + len - 4] | p[c + len - 3] << 8 | p[c + len - 2] << 16 | (u32)p[c + len - 1] << 24;
+	return *isize > GZ_BGZF_MAX_ISIZE ? GZ_B_BIG : GZ_B_OK;
+}
+// the whole chain (one thread): members m[0, *nm), or GZ_B_* with *at = the compressed offset where the chain broke
+SSQ_HD int gz_bgzf_chain(const uint8_t *p, bz_u64 n, GzMember *m, bz_u64 cap, bz_u64 *nm, bz_u64 *at)
+{
+	bz_u64 c = 0, t = 0, k = 0;
+	while (c < n) {
+		u32 cs, is;
+		const int r = gz_bgzf_member(p, n, c, &cs, &is);
+		if (r) { *nm = k; *at = c; return r; }
+		if (k == cap) { *nm = k; *at = c; return GZ_B_CAP; }
+		m[k].coff = c; m[k].toff = t; m[k].csize = cs; m[k].isize = is;
+		++k; c += cs; t += is;
+	}
+	*nm = k; *at = n;
+	return GZ_B_OK;
+}
+static inline const char *gz_bgzf_why(int r)
+{
+	return r == GZ_B_NOHDR ? "no gzip member header where the BSIZE chain lands" : r == GZ_B_NOBSIZE ? "a member without a BGZF BSIZE field" :
+	       r == GZ_B_TRUNC ? "a truncated member" : r == GZ_B_BIG ? "a member of more than 64 KB of text" : "more members than the table holds";
+}
+
+// a member's symbols (all literal bytes: a member references nothing before it) -> its text
+SSQ_HD void gz_bgzf_emit(const uint16_t *slot, u32 len, uint8_t *out, u32 t, u32 nt) { for (u32 o = t; o < len; o += nt) out[o] = (uint8_t)slot[o]; }
+// Backend of the member-parallel path: the members m[k0, k0 + k) decode into slots 0 .. k-1 and their text goes to out + toff
+struct GzBgzfBackend {
+	virtual ~GzBgzfBackend() {}
+	virtual int decode(const GzMember *m, int k, GzChunk *ch, GzEvent *ev) = 0;                    // ch/ev: host mirrors
+	virtual int emit(const GzMember *m, int k) = 0;                                                // slots -> text
+	virtual int crc(const std::vector<bz_u64> &off, const std::vector<u32> &len, std::vector<u32> &out) = 0; // pieces of the text
+};
+// the members, GZ_MAXCH at a time: 0, or SSQ_EDATA with *err_at = the compressed offset of the first member that fails
+static inline int gz_bgzf_members(GzBgzfBackend &be, const std::vector<GzMember> &m, bz_u64 *err_at)
+{
+	std::vector<GzChunk> ch; std::vector<GzEvent> ev;
+	std::vector<bz_u64> poff; std::vector<u32> plen, pc; std::vector<int> pm;
+	int rc;
+	for (size_t b = 0; b < m.size(); b += GZ_MAXCH) {
+		const int k = (int)(m.size() - b < GZ_MAXCH ? m.size() - b : GZ_MAXCH);
+		ch.assign(k, GzChunk()); ev.assign((size_t)k * GZ_EVCAP, GzEvent());
+		for (int i = 0; i < k; ++i) { ch[i].start.bit = ch[i].start.hdr = 0; ch[i].start.mode = GZ_M_FIRST; ch[i].stop = GZ_NONE; }
+		if ((rc = be.decode(m.data() + b, k, ch.data(), ev.data()))) return rc;
+		poff.clear(); plen.clear(); pm.clear();
+		for (int i = 0; i < k; ++i) {
+			const GzChunk &c = ch[i]; const GzEvent &E = ev[(size_t)i * GZ_EVCAP]; const GzMember &M = m[b + i];
+			// one member, decoded to its end, nothing after it: its trailer is the member's last 8 bytes, its ISIZE the chain's
+			if (c.status != GZ_S_EOS || c.n_ev != 1 || E.out != c.len || c.len != M.isize || E.at + 8 != M.csize) { *err_at = M.coff; return SSQ_EDATA; }
+			for (u32 x = 0; x < M.isize; x += GZ_CRC_PIECE) { poff.push_back(M.toff + x); plen.push_back(M.isize - x < GZ_CRC_PIECE ? M.isize - x : GZ_CRC_PIECE); pm.push_back(i); }
+		}
+		if ((rc = be.emit(m.data() + b, k)) || (rc = be.crc(poff, plen, pc))) return rc;
+		size_t p = 0;
+		for (int i = 0; i < k; ++i) {
+			u32 crc = 0;
+			for (; p < poff.size() && pm[p] == i; ++p) crc = bz_multmodp(bz_x8n(plen[p]), crc) ^ pc[p];
+			if (crc != ev[(size_t)i * GZ_EVCAP].crc) { *err_at = m[b + i].coff; return SSQ_EDATA; }
+		}
+	}
+	return SSQ_OK;
+}
+
 // a whole stream in p[0, n): windows until the end of the stream; emit(text) takes each window's text out of the backend
 template <class Emit>
 static inline int gz_run(GzBackend &be, GzState &S, const uint8_t *p, bz_u64 n, bz_u64 chunk_bytes, Emit emit, bz_u64 *err_at)

@@ -8,7 +8,7 @@
 #   b200_bam   : + SSQ_FUSE_BAM and $SAMBAMBA = speedseq_b200/bin/sambamba: the main records never exist as text
 #   b200_bamz  : b200_bam + SSQ_BGZF_GPU=1: the shim's sort compresses the sorted BAM on the device
 #   b200_view  : the default unfused shims, $SAMBAMBA = speedseq_b200/bin/sambamba with SSQ_SAM2BAM_GPU=1: every `view -S` (main and
-#                both side streams) converts its SAM on the device into sorted runs for the shim's sort; `index` goes to the real one
+#                both side streams) converts its SAM on the device into sorted runs for the shim's sort; `index` runs on the device too
 set -e
 MODE=${1:-oracle}; REF=${2:?usage: tools/run_config1.sh MODE SPEEDSEQ_CHECKOUT [WORKDIR]}; W=${3:-/tmp/ssq_config1}
 ROOT=$(cd "$(dirname "$0")/.." && pwd)
