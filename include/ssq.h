@@ -412,6 +412,30 @@ int ssq_bai_build(ssq_bai_t *b, const void *bam, size_t len, void **bai_out, siz
 int ssq_bai_times(const ssq_bai_t *b, float ms[3]);
 void *ssq_bai_stream(ssq_bai_t *b);                 /* cudaStream_t of the object, for event timing */
 void ssq_bai_free(ssq_bai_t *b);
+/* The merge of coordinate-sorted BAM files on the device (csrc/ssq_merge.cu): the records in the order `sambamba merge out.bam
+ * in1.bam in2.bam ...` (0.5.9) writes them, and its merged header — the calls of `speedseq realign` with several libraries
+ * (speedseq:2002-2009).  The inputs stream through windows of whole BGZF members of at most window_bytes compressed bytes each
+ * (0 = 32 MB), so they need not fit in device memory.  The rules and what is refused are at the head of csrc/ssq_merge.cuh; in
+ * short, SSQ_EDATA for an input that is not BGZF or does not inflate, SSQ_EFORMAT (the file and record in ssq_last_error()) for
+ * headers that do not merge the way the device merges them (not all SO:coordinate, @HD lines or @SQ dictionaries that differ, an
+ * @RG / @PG ID carried by two different lines, other header lines), a refID outside the header and records out of coordinate
+ * order, SSQ_EINVAL for fewer than two inputs.  One host thread at a time per object; without a usable GPU create returns
+ * SSQ_ENOGPU. */
+typedef struct ssq_merge ssq_merge_t;
+/* the output, piece by piece in file order; nonzero stops the merge (SSQ_EIO) */
+typedef int (*ssq_merge_sink_t)(void *ctx, const void *p, size_t n);
+int ssq_merge_create(int device, size_t window_bytes, ssq_merge_t **out);
+/* paths[0, n_in): the inputs.  sink receives the merged file without its end-of-file block: the uncompressed BAM ("BAM\1", header,
+ * reference table, records) when z is null; with z, BGZF members at `level` compressed on the device, the header in blocks of its
+ * own.  Something may have reached sink before an error.  *n_records (may be null): records written. */
+int ssq_merge_run(ssq_merge_t *m, const char *const *paths, int n_in, ssq_bgzf_t *z, int level, ssq_merge_sink_t sink, void *ctx, uint64_t *n_records);
+/* the merged header text alone (`sambamba merge -H`), read on the host; the refusals of the header.  Free with ssq_free */
+int ssq_merge_header(const char *const *paths, int n_in, char **text);
+/* the last run in ms of host clock around synchronised work: 0 windows (read, copy in, inflate, record walk, keys), 1 the host heap,
+ * 2 gathers and the output (compression on the device, the copy back and the sink included) */
+int ssq_merge_times(const ssq_merge_t *m, float ms[3]);
+void *ssq_merge_stream(ssq_merge_t *m);             /* cudaStream_t of the object, for event timing */
+void ssq_merge_free(ssq_merge_t *m);
 /* the sorted runs of consecutive batches -> one sorted record stream (stable: equal keys keep batch order); free with ssq_free */
 int ssq_bam_merge_runs(int n_runs, const void *const *runs, const size_t *lens, void **out, size_t *out_len);
 

@@ -419,3 +419,60 @@ class SSQ:
 
     def bai_free(self, b):
         self.lib.ssq_bai_free(b)
+
+    # ---- merge of sorted BAM files on the device (ssq_merge_*) ----
+    _MERGE_SINK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
+
+    def merge_create(self, device=0, window_bytes=0):
+        L = self.lib
+        L.ssq_merge_create.argtypes = [C.c_int, C.c_size_t, C.c_void_p]
+        L.ssq_merge_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, self._MERGE_SINK, C.c_void_p, C.c_void_p]
+        L.ssq_merge_header.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        L.ssq_merge_times.argtypes = [C.c_void_p, C.c_void_p]
+        L.ssq_merge_stream.restype = C.c_void_p
+        L.ssq_merge_stream.argtypes = [C.c_void_p]
+        L.ssq_merge_free.argtypes = [C.c_void_p]
+        L.ssq_free.argtypes = [C.c_void_p]
+        h = C.c_void_p()
+        self.ck(L.ssq_merge_create(C.c_int(device), C.c_size_t(window_bytes), C.byref(h)), "ssq_merge_create")
+        return h
+
+    def merge_run(self, m, paths, z=None, level=6):
+        """the merge of the files `paths` -> (rc, output bytes, records); the output is the uncompressed BAM without z, else BGZF
+        members without the end-of-file block; rc is 0, SSQ_EINVAL (-4), SSQ_EFORMAT (-8) or SSQ_EDATA (-9), whose message
+        ssq_last_error() holds"""
+        parts = []
+
+        def put(ctx, p, n):
+            parts.append(C.string_at(p, n))
+            return 0
+        sink = self._MERGE_SINK(put)
+        arr = (C.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
+        n = C.c_uint64(0)
+        rc = self.lib.ssq_merge_run(m, arr, len(paths), z, C.c_int(level), sink, None, C.byref(n))
+        if rc not in (0, -4, -8, -9):
+            self.ck(rc, "ssq_merge_run")
+        return rc, b"".join(parts) if rc == 0 else b"", int(n.value)
+
+    def merge_header(self, paths):
+        """the merged header text (`sambamba merge -H`) -> (rc, text)"""
+        out = C.c_void_p()
+        arr = (C.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
+        rc = self.lib.ssq_merge_header(arr, len(paths), C.byref(out))
+        if rc:
+            return rc, b""
+        data = C.string_at(out)
+        self.lib.ssq_free(out)
+        return 0, data
+
+    def merge_times(self, m):
+        """ms of the last run: (windows: read, inflate, walk, keys; the host heap; gathers and output)"""
+        ms = (C.c_float * 3)()
+        self.ck(self.lib.ssq_merge_times(m, ms), "ssq_merge_times")
+        return tuple(ms)
+
+    def merge_stream(self, m):
+        return self.lib.ssq_merge_stream(m)
+
+    def merge_free(self, m):
+        self.lib.ssq_merge_free(m)

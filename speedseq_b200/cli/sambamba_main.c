@@ -19,7 +19,13 @@
  *          byte-identical to sambamba's index; -t and -p change nothing).  -c / --check-bins, -C / CRAM, other options, input that
  *          is not BGZF, input the device refuses (its rules: csrc/ssq_bai.cuh) and no usable GPU go to the real sambamba after one
  *          stderr line naming the reason; after `sort`, such a file is indexed by the real sambamba's `index`.
- * Everything else — other subcommands (merge, ...), and view / sort whose stdin is ordinary SAM / BAM (without
+ *   merge: with SSQ_MERGE_GPU=1, `merge [-t N] [-l N] [-p] out.bam in1.bam in2.bam ...` (speedseq:2002-2009) runs on the device
+ *          (ssq_merge_run: sambamba's record order and merged header; compressed on -t threads, or on the device with
+ *          SSQ_BGZF_GPU=1) into a temporary file beside out.bam, renamed at the end, then out.bam.bai as after `sort`; `merge -H`
+ *          prints the merged header, read on the host.  Other options, fewer than two inputs, and inputs the device refuses (its
+ *          rules: csrc/ssq_merge.cuh; found before or during the merge) and no usable GPU go to the real sambamba after one
+ *          stderr line naming the reason, the temporary file removed.  SSQ_MERGE_WINDOW: compressed bytes per input window.
+ * Everything else — other subcommands, `merge` without SSQ_MERGE_GPU=1, and view / sort whose stdin is ordinary SAM / BAM (without
  * SSQ_SAM2BAM_GPU, the splitter and discordant streams, speedseq:444-448) — goes to the real sambamba named by SSQ_SAMBAMBA_REAL
  * (or `sambamba.real` next to this executable) with the bytes already read handed on, so one SAMBAMBA= line serves the whole
  * script. */
@@ -169,12 +175,21 @@ static void merge_sources(src_t *s, int n_src, sink_fn sink, void *ctx)
 }
 
 /* ---- BGZF output on several threads, or on the device (SSQ_BGZF_GPU=1) ---- */
-typedef struct { FILE *fp; const uint8_t *buf; size_t n; int threads, level; ssq_bgzf_t *z; } flush_t;
-typedef struct { FILE *fp; uint8_t *buf, *alt; size_t n, cap; int threads, level; ssq_bgzf_t *z; pthread_t bg; int bg_live; flush_t job; } bgzf_out_t;
-static void write_member_bytes(FILE *fp, void *p, size_t n)
+/* err: null = a failed write or compression ends the process; else it sets *err and the caller cleans up (merge: its temporary file) */
+typedef struct { FILE *fp; const uint8_t *buf; size_t n; int threads, level; ssq_bgzf_t *z; int *err; } flush_t;
+typedef struct { FILE *fp; uint8_t *buf, *alt; size_t n, cap; int threads, level; ssq_bgzf_t *z; pthread_t bg; int bg_live; flush_t job; int *err; } bgzf_out_t;
+static void flush_fail(const flush_t *f, const char *what)
 {
-	if (fwrite(p, 1, n, fp) != n) { perror("sambamba (GPU shim): write"); exit(1); }
+	fprintf(stderr, "sambamba (GPU shim): %s\n", what);
+	if (!f->err) exit(1);
+	*f->err = 1;
+}
+static int write_member_bytes(const flush_t *f, void *p, size_t n)
+{
+	const int bad = fwrite(p, 1, n, f->fp) != n;
 	ssq_free(p);
+	if (bad) { char m[300]; snprintf(m, sizeof m, "write: %s", strerror(errno)); flush_fail(f, m); }
+	return bad;
 }
 typedef struct { const uint8_t *in; size_t n; int level; void *out; size_t out_len; int rc; } job_t;
 static void *job_main(void *a) { job_t *j = (job_t*)a; j->rc = ssq_bgzf_compress(j->in, j->n, j->level, 0, &j->out, &j->out_len); return 0; }
@@ -188,8 +203,8 @@ static void *flush_main(void *a) /* one buffer: compressed in slices on `threads
 	size_t per, at = 0;
 	if (f->z) { /* the whole buffer in one call on the device */
 		void *out = 0; size_t len = 0;
-		if (ssq_bgzf_deflate(f->z, f->buf, f->n, f->level, 0, &out, &len)) { fprintf(stderr, "sambamba (GPU shim): BGZF compression on the device (SSQ_BGZF_GPU=1) failed: %s\n", ssq_last_error()); exit(1); }
-		write_member_bytes(f->fp, out, len);
+		if (ssq_bgzf_deflate(f->z, f->buf, f->n, f->level, 0, &out, &len)) { char m[600]; snprintf(m, sizeof m, "BGZF compression on the device (SSQ_BGZF_GPU=1) failed: %s", ssq_last_error()); flush_fail(f, m); return 0; }
+		write_member_bytes(f, out, len);
 		return 0;
 	}
 	per = ((f->n / blk + (size_t)nj) / (size_t)nj) * blk;
@@ -198,10 +213,9 @@ static void *flush_main(void *a) /* one buffer: compressed in slices on `threads
 	for (k = 1; k < nj; ++k) pthread_create(&th[k], 0, job_main, &jobs[k]);
 	job_main(&jobs[0]);
 	for (k = 1; k < nj; ++k) pthread_join(th[k], 0);
-	for (k = 0; k < nj; ++k) {
-		if (jobs[k].rc) { fprintf(stderr, "sambamba (GPU shim): BGZF compression failed: %s\n", ssq_last_error()); exit(1); }
-		write_member_bytes(f->fp, jobs[k].out, jobs[k].out_len);
-	}
+	for (k = 0; k < nj; ++k) if (jobs[k].rc) { char m[600]; snprintf(m, sizeof m, "BGZF compression failed: %s", ssq_last_error()); flush_fail(f, m); break; }
+	if (k < nj) { for (k = 0; k < nj; ++k) ssq_free(jobs[k].out); return 0; }
+	for (k = 0; k < nj; ++k) if (write_member_bytes(f, jobs[k].out, jobs[k].out_len)) { while (++k < nj) ssq_free(jobs[k].out); break; }
 	return 0;
 }
 static void bgzf_wait(bgzf_out_t *o) { if (o->bg_live) { pthread_join(o->bg, 0); o->bg_live = 0; } }
@@ -212,7 +226,7 @@ static void bgzf_flush(bgzf_out_t *o)
 	uint8_t *t;
 	if (!o->n) return;
 	bgzf_wait(o);
-	o->job.fp = o->fp; o->job.buf = o->buf; o->job.n = o->n; o->job.threads = o->threads; o->job.level = o->level; o->job.z = o->z;
+	o->job.fp = o->fp; o->job.buf = o->buf; o->job.n = o->n; o->job.threads = o->threads; o->job.level = o->level; o->job.z = o->z; o->job.err = o->err;
 	if (pthread_create(&o->bg, 0, flush_main, &o->job)) flush_main(&o->job); else o->bg_live = 1;
 	t = o->buf; o->buf = o->alt; o->alt = t;
 	o->n = 0;
@@ -478,6 +492,73 @@ static int sort_index(const char *out_fn)
 	}
 }
 
+/* ---- `merge` on the device (SSQ_MERGE_GPU=1): ssq_merge_run into a temporary file beside out.bam, renamed at the end ---- */
+typedef struct { bgzf_out_t *o; FILE *fp; int calls, err; } merge_out_t;
+static int merge_put(void *ctx, const void *p, size_t n)
+{
+	merge_out_t *m = (merge_out_t*)ctx;
+	if (m->err) return 1;
+	if (m->fp) { if (fwrite(p, 1, n, m->fp) != n) { fprintf(stderr, "sambamba (GPU shim): write: %s\n", strerror(errno)); m->err = 1; } return m->err; } /* BGZF members made on the device */
+	bgzf_put(m->o, (const uint8_t*)p, n);
+	if (!m->calls++) bgzf_flush(m->o); /* the first piece is the header: blocks of its own, as sambamba writes it */
+	return m->err; /* set by a background write or compression that failed */
+}
+static void merge_refuse(char **argv, const char *tmp, const char *why)
+{
+	if (tmp) unlink(tmp);
+	fprintf(stderr, "sambamba (GPU shim): merge: %s; running the real sambamba\n", why);
+	exec_real(argv, "this `merge`");
+}
+static int merge_main(int argc, char **argv)
+{
+	const char *g = getenv("SSQ_MERGE_GPU"), *out_fn = 0, *dv = getenv("SSQ_DEVICE"), *w = getenv("SSQ_MERGE_WINDOW");
+	const char **in = (const char**)calloc((size_t)argc, sizeof(char*));
+	int n_in = 0, threads = 1, level = 6, header_only = 0, i, rc;
+	char *text = 0, why[1200], tmp[4096];
+	ssq_merge_t *m = 0;
+	ssq_bgzf_t *z = 0;
+	bgzf_out_t o;
+	merge_out_t mo;
+	if (!g || strcmp(g, "1")) exec_real(argv, "`merge`");
+	for (i = 2; i < argc; ++i) {
+		if ((!strcmp(argv[i], "-t") || !strcmp(argv[i], "--nthreads")) && i + 1 < argc) threads = atoi(argv[++i]);
+		else if (!strncmp(argv[i], "--nthreads=", 11)) threads = atoi(argv[i] + 11);
+		else if ((!strcmp(argv[i], "-l") || !strcmp(argv[i], "--compression-level")) && i + 1 < argc) level = atoi(argv[++i]);
+		else if (!strncmp(argv[i], "--compression-level=", 20)) level = atoi(argv[i] + 20);
+		else if (!strcmp(argv[i], "-p") || !strcmp(argv[i], "--show-progress")) {}
+		else if (!strcmp(argv[i], "-H") || !strcmp(argv[i], "--header")) header_only = 1;
+		else if (argv[i][0] == '-' && argv[i][1]) { snprintf(why, sizeof why, "option %s is not on the GPU", argv[i]); merge_refuse(argv, 0, why); }
+		else if (!out_fn) out_fn = argv[i];
+		else in[n_in++] = argv[i];
+	}
+	if (!out_fn || n_in < 2) merge_refuse(argv, 0, "it needs an output and at least two inputs");
+	if ((rc = ssq_merge_header(in, n_in, &text))) merge_refuse(argv, 0, ssq_last_error());
+	if (header_only) { fputs(text, stdout); ssq_free(text); return 0; } /* `merge -H`: the merged header, on the host */
+	ssq_free(text);
+	if (ssq_merge_create(dv && dv[0] ? atoi(dv) : 0, w && atoll(w) > 0 ? (size_t)atoll(w) : 0, &m)) { snprintf(why, sizeof why, "no usable GPU: %s", ssq_last_error()); merge_refuse(argv, 0, why); }
+	if (g = getenv("SSQ_BGZF_GPU"), g && !strcmp(g, "1") && ssq_bgzf_create(dv && dv[0] ? atoi(dv) : 0, &z)) { snprintf(why, sizeof why, "SSQ_BGZF_GPU=1 asks for BGZF compression on the GPU, but: %s", ssq_last_error()); merge_refuse(argv, 0, why); }
+	snprintf(tmp, sizeof tmp, "%s.ssq_merge_%ld.tmp", out_fn, (long)getpid());
+	memset(&o, 0, sizeof o); memset(&mo, 0, sizeof mo);
+	if (!(o.fp = fopen(tmp, "wb"))) { fprintf(stderr, "sambamba (GPU shim): cannot create %s: %s\n", tmp, strerror(errno)); return 1; }
+	o.threads = threads < 1 ? 1 : threads > 64 ? 64 : threads; o.level = level;
+	if (z) mo.fp = o.fp;
+	else {
+		o.cap = (size_t)0xff00 * 256 * (size_t)o.threads; o.buf = (uint8_t*)malloc(o.cap); o.alt = (uint8_t*)malloc(o.cap);
+		if (!o.buf || !o.alt) { fprintf(stderr, "sambamba (GPU shim): out of memory\n"); unlink(tmp); return 1; }
+		mo.o = &o; o.err = &mo.err;
+	}
+	rc = ssq_merge_run(m, in, n_in, z, level, merge_put, &mo, 0);
+	if (!z) { if (!mo.err) bgzf_flush(&o); bgzf_wait(&o); }
+	if (mo.err) { fclose(o.fp); unlink(tmp); fprintf(stderr, "sambamba (GPU shim): merge: %s could not be written; nothing is left of it\n", tmp); return 1; }
+	if (rc) { fclose(o.fp); snprintf(why, sizeof why, "the device does not merge these files: %s", ssq_last_error()); merge_refuse(argv, tmp, why); }
+	{ void *eofb = 0; size_t el = 0; if (ssq_bgzf_compress("", 0, level, 1, &eofb, &el) || fwrite(eofb, 1, el, o.fp) != el) { fprintf(stderr, "sambamba (GPU shim): cannot write %s\n", tmp); unlink(tmp); return 1; } ssq_free(eofb); }
+	if (fclose(o.fp) || rename(tmp, out_fn)) { fprintf(stderr, "sambamba (GPU shim): cannot write %s: %s\n", out_fn, strerror(errno)); unlink(tmp); return 1; }
+	ssq_merge_free(m);
+	if (z) ssq_bgzf_free(z);
+	free(o.buf); free(o.alt); free(in);
+	return sort_index(out_fn); /* out.bam.bai, as sambamba's merge writes it */
+}
+
 int main(int argc, char **argv)
 {
 	head_t h;
@@ -534,6 +615,7 @@ int main(int argc, char **argv)
 		return sort_index(out_fn);
 	}
 	if (!strcmp(argv[1], "index")) return index_main(argc, argv);
+	if (!strcmp(argv[1], "merge")) return merge_main(argc, argv);
 	exec_real(argv, "this subcommand");
 	return 1;
 }

@@ -256,7 +256,9 @@ static inline int bai_header(const uint8_t *t, bz_u64 have, bz_u64 total, bz_u64
 // the order sambamba 0.5.9 writes one reference's bins in: its D associative array (druntime's chained hash table: 4 buckets,
 // hash of a uint = its value, new keys at the tail of their bucket, rehashed to the next size of a prime list when it holds more
 // than 4 keys per bucket, the old keys moved last to first; iterated bucket by bucket).  keys: the bins in the order their first chunks were made
-static inline void bai_aa_order(const std::vector<u32> &keys, std::vector<int> &order)
+// (the same table keyed by strings orders the merged header's read-group and program IDs, ssq_merge.cuh)
+template <class K>
+static inline void bai_aa_order(const std::vector<K> &keys, std::vector<int> &order)
 {
 	static const bz_u64 primes[] = {31, 97, 389, 1543, 6151, 24593, 98317, 393241, 1572869};
 	std::vector<std::vector<int>> bk(4);

@@ -9,6 +9,7 @@
 #include <vector>
 #include <zlib.h>
 #include "ssq_host.h"
+#include "ssq_samhdr.h"
 
 extern "C" int ssq_mem_batch_sam(const ssq_index_t *idx, const ssq_opts_t *opt, int n_reads, const char *const *names, const char *const *seqs, const char *const *quals,
                                  const char *const *comments, int64_t n_processed, int paired, const ssq_pestat_t *pes0, const char *rg_id, int verbose, char **sam_out, size_t *sam_len, size_t *read_sam_off)
@@ -90,21 +91,8 @@ extern "C" int ssq_bgzf_compress(const void *in_, size_t n, int level, int with_
 
 // The header text as `sambamba view -S | sambamba sort` leaves it (speedseq:440-441): "@HD VN:1.3 SO:coordinate" first (any @HD of the
 // input replaced), and the tags of @SQ / @RG / @PG lines in sambamba's fixed field order (v0.5.9: SQ: SN LN AS M5 SP UR; RG: ID CN DS DT FO KS
-// LB PG PI PL PU SM; PG: ID PN CL PP VN), tags it does not know after them in input order.  Other lines (@CO) pass through.
-static void reorder_tags(const std::string &line, std::string &out)
-{
-	static const char *SQ[] = {"SN", "LN", "AS", "M5", "SP", "UR", 0}, *RG[] = {"ID", "CN", "DS", "DT", "FO", "KS", "LB", "PG", "PI", "PL", "PU", "SM", 0}, *PG[] = {"ID", "PN", "CL", "PP", "VN", 0};
-	const char **ord = !line.compare(0, 3, "@SQ") ? SQ : !line.compare(0, 3, "@RG") ? RG : !line.compare(0, 3, "@PG") ? PG : 0;
-	if (!ord) { out += line; out += '\n'; return; }
-	std::vector<std::string> f;
-	for (size_t p = 0;;) { const size_t e = line.find('\t', p); f.push_back(line.substr(p, e == std::string::npos ? e : e - p)); if (e == std::string::npos) break; p = e + 1; }
-	std::vector<char> used(f.size(), 0);
-	out += f[0];
-	for (int k = 0; ord[k]; ++k)
-		for (size_t i = 1; i < f.size(); ++i) if (!used[i] && f[i].size() >= 3 && f[i][2] == ':' && !f[i].compare(0, 2, ord[k])) { out += '\t'; out += f[i]; used[i] = 1; }
-	for (size_t i = 1; i < f.size(); ++i) if (!used[i]) { out += '\t'; out += f[i]; }
-	out += '\n';
-}
+// LB PG PI PL PU SM; PG: ID PN CL PP VN), tags it does not know after them in input order (reorder_tags, ssq_samhdr.h).  Other
+// lines (@CO) pass through.
 extern "C" int ssq_bam_header_text(const char *sam_header_text, int sorted, char **out)
 {
 	if (!out) return SSQ_EINVAL;
