@@ -17,6 +17,7 @@
 #include <cuda_runtime.h>
 #include <cub/cub.cuh>
 #include <cub/device/device_merge.cuh>
+#include <map>
 #include <mutex>
 #include <condition_variable>
 #include <stdio.h>
@@ -1349,6 +1350,22 @@ __global__ void k_dup_mark(u64 n, const u32 *__restrict__ idx, const u64 *__rest
 // ===================================================================== host-side launch code ====
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { ssq_set_error("%s:%d: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); return SSQ_ECUDA; } } while (0)
 
+// A kernel's dynamic shared-memory limit belongs to the kernel (on each device), not to the batch that launches it: aligner objects
+// on other host threads launch the same kernel concurrently.  So it only ever grows — a batch of short reads that set its own
+// smaller need made a concurrent launch for long reads fail ("invalid argument").
+static int raise_smem_limit(const void *fn, size_t bytes)
+{
+	static std::mutex mu;
+	static std::map<std::pair<const void*, int>, size_t> limit;
+	int dev = 0;
+	CK(cudaGetDevice(&dev));
+	std::lock_guard<std::mutex> g(mu);
+	size_t &cur = limit[std::make_pair(fn, dev)];
+	if (bytes <= cur) return SSQ_OK;
+	CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+	cur = bytes;
+	return SSQ_OK;
+}
 
 struct ssq_batch {
 	const ssq_index *idx;
@@ -1594,7 +1611,7 @@ static int run_smem(ssq_batch *b)
 	if (b->pool_cap == 0) b->pool_cap = (u64)n * 48 + 4096;
 	if (b->scratch.need(scratch_entries * sizeof(Intv))) return SSQ_ENOMEM;
 	if (b->intv_off.need((size_t)(n + 1) * 8) || b->intv_cnt.need((size_t)(n + 1) * 4) || b->l_rep.need((size_t)(n + 1) * 4) || b->misc.need(sizeof(Misc)) || b->xovf.need((size_t)(n + 1) * 4)) return SSQ_ENOMEM;
-	if (variant == 0) CK(cudaFuncSetAttribute(k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	if (variant == 0) { const int rc = raise_smem_limit((const void*)k_smem, smem); if (rc) return rc; }
 	for (int attempt = 0; attempt < 6; ++attempt) {
 		if (b->pool.need(b->pool_cap * sizeof(Intv))) return SSQ_ENOMEM;
 		CK(cudaMemsetAsync(b->misc.p, 0, sizeof(Misc), b->st));
@@ -1789,8 +1806,7 @@ static int run_extend(ssq_batch *b)
 		CK(cudaFuncSetAttribute(k_ext_run<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 131072 + 8192));
 		CK(cudaFuncSetAttribute(k_ext_run<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 131072 + 8192));
 		const size_t rsmem = (size_t)64 * (b->max_len + 2) * 4;
-		CK(cudaFuncSetAttribute(k_ext_retry<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem));
-		CK(cudaFuncSetAttribute(k_ext_retry<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem));
+		if ((rc = raise_smem_limit((const void*)k_ext_retry<0>, rsmem)) || (rc = raise_smem_limit((const void*)k_ext_retry<1>, rsmem))) return rc;
 		const cudaEvent_t es0 = b->evx[0], es1 = b->evx[1];
 		for (int round = 0;; ++round) {
 			for (int dir = 0; dir < 2; ++dir) {
@@ -2067,7 +2083,7 @@ extern "C" int ssq_sw_extend_batch(const ssq_opts_t *opt, int device, uint64_t n
 	CK(cudaMemcpy(dtb.p, tbuf, tbuf_len, cudaMemcpyHostToDevice));
 	const int threads = 64;
 	const size_t smem = (size_t)threads * (qmax + 2) * 4;
-	CK(cudaFuncSetAttribute(k_sw_tasks, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	if ((rc = raise_smem_limit((const void*)k_sw_tasks, smem))) return rc;
 	k_sw_tasks<<<(unsigned)((n + threads - 1) / threads), threads, smem>>>(*opt, n, dt.as<ssq_sw_task_t>(), dq.as<uint8_t>(), dtb.as<uint8_t>(), dout.as<ssq_sw_result_t>());
 	CK(cudaGetLastError());
 	CK(cudaMemcpy(out, dout.p, n * sizeof(ssq_sw_result_t), cudaMemcpyDeviceToHost));
